@@ -1,4 +1,4 @@
-/* bevbert_b200 C ABI — the sm_100a kernels behind the BEVBert hybrid-map encoder hot path.
+/* bevbert_b200 C ABI — the sm_90a kernels behind the BEVBert hybrid-map encoder hot path.
  *
  * Conventions (SURVEY.md 8b):
  *   - every pointer is a DEVICE pointer on the current CUDA device unless the name ends in _host;
@@ -32,7 +32,7 @@ void bb_reset_launch_count(void);
 int bb_set_drop_salt_ptr(const uint64_t* device_word);
 
 /* ---------------------------------------------------------------------------------------------
- * Batched bf16 GEMM on tcgen05 tensor cores, TMA-fed, fp32 accumulation in TMEM.
+ * Batched bf16 GEMM on wgmma tensor cores, TMA-fed, fp32 accumulation in registers.
  *   D[b] = epi( alpha * A[b] (M x K) * B[b]^T (N x K) )
  * Operand element (m,k) of A lives at  A + b1*a_s1 + b2*a_s2 + (a_mn ? k*lda + m : m*lda + k),
  * operand element (n,k) of B lives at  B + b1*b_s1 + b2*b_s2 + (b_mn ? k*ldb + n : n*ldb + k).
@@ -65,7 +65,7 @@ typedef struct bb_gemm_args {
   uint32_t drop_thresh; /*   keep iff rng(seed, output element offset) >= thresh; 0 = no dropout   */
   float drop_scale;     /*   1/(1-p)                                                              */
   const void* add_in; /* bf16, same strides as D, or NULL: result += add_in (last) */
-  int32_t block_n;   /* 0 = pick automatically; else N tile (multiple of 16, of 64 when b_mn) */
+  int32_t block_n;   /* 0 = pick automatically; else a tile-width hint (16..256, multiple of 16, of 64 when b_mn): <= 64 selects 64-wide N tiles, larger 128-wide */
 } bb_gemm_args;
 
 int bb_gemm_bf16(const bb_gemm_args* args, void* stream);
@@ -216,8 +216,8 @@ int bb_softmax_xent(const float* logits, const int64_t* labels, int64_t rows, in
 
 /* ---------------------------------------------------------------------------------------------
  * Fused attention scores (keys per row <= 512, head dim 64): the 128 x nk product of one (sample, head, query
- * tile) goes tcgen05.mma -> TMEM and the row softmax / softmax-backward runs in the epilogue; no fp32 score
- * matrix in HBM.  A = Q (mode 0) or dO (mode 1): element (b,h,q,d) at A + b*a_s2 + h*a_s1 + q*lda + d;
+ * tile) is formed by wgmma in registers, 64 keys at a time, and the row softmax / softmax-backward runs on the
+ * accumulators; no fp32 score matrix in HBM.  A = Q (mode 0) or dO (mode 1): element (b,h,q,d) at A + b*a_s2 + h*a_s1 + q*lda + d;
  * Bm = K (mode 0) or V (mode 1) likewise with nk rows.  P / Pd / Pin / dS are bf16 (B,H,nq,ldp).
  *   mode 0: P = softmax(alpha*A Bm^T + kmask + bias), Pd = dropout(P) (Pd may be NULL)
  *   mode 1: dS = Pin o (g - sum_k Pin g) * out_scale with g = dropout-mask(A Bm^T); dbias (B,nq,nk) f32 += unscaled
@@ -267,11 +267,10 @@ typedef struct bb_flash_args {
 } bb_flash_args;
 int bb_flash_fwd(const bb_flash_args* args, void* stream);
 /* Which core serves bb_flash_fwd / bb_flash_bwd: 0 = always the warp-level mma.sync kernels (csrc/attn_flash.cu),
- * 1 (default, or env BB_ATTN_TC) = the tcgen05 / TMA kernels (csrc/attn_tc.cu) when nk >= 64 and bias == NULL,
- * 2 = the tcgen05 kernels whenever they support the call (any nk; tests).  Returns the previous mode. */
+ * 1 (default, or env BB_ATTN_TC) = the wgmma / TMA kernels (csrc/attn_tc.cu) when nk >= 64 and bias == NULL,
+ * 2 = the wgmma kernels whenever they support the call (any nk; tests).  Returns the previous mode. */
 int bb_set_attn_tc(int mode);
-/* Debug: when device_buf is not NULL the tcgen05 forward kernel writes 8 %globaltimer stamps per CTA (first 256 CTAs):
- * [0] start, [1] key mask staged, [2] S ready, [3] row max done, [4] P written, [5] O ready, [6] rows stored. */
+/* Kept for ABI compatibility: accepts and ignores a trace buffer (the wgmma attention kernels record no trace). */
 int bb_attn_tc_trace(long long* device_buf);
 int bb_flash_bwd(const bb_flash_args* args, void* stream);
 

@@ -52,20 +52,6 @@ for name, b, nq, nk, cross, p in [("bev self 441", B, 441, 441, False, 0.1), ("l
     tf = timeit(lambda: K.flash_fwd(q, k, v, b, H, nq, nk, ldq, ldk, ldv, kmask, None, drop))
     tb = timeit(lambda: K.flash_bwd(q, k, v, o, lse, dout, b, H, nq, nk, ldq, ldk, ldv, kmask, None, drop,
                                     out=(dq, Hd, dk, Hd, dv, Hd)))
-    if os.environ.get("ATTN_TRACE"):
-        import bevbert_b200._lib as L
-        buf = torch.zeros(256 * 8, dtype=torch.int64, device="cuda")
-        L.load().bb_attn_tc_trace(buf.data_ptr())
-        K.flash_fwd(q, k, v, b, H, nq, nk, ldq, ldk, ldv, kmask, None, drop)
-        torch.cuda.synchronize()
-        L.load().bb_attn_tc_trace(None)
-        t = buf.view(256, 8).cpu().double()
-        t = t[t[:, 6] > 0]
-        if len(t):
-            d = (t[:, 1:7] - t[:, 0:6]).mean(0)
-            first = t[:148]
-            print("   trace ns (mean over %d CTAs): stage-mask %.0f | wait-S %.0f | pass1 %.0f | pass2 %.0f | wait-O %.0f | store %.0f | total %.0f ; first-wave span %.0f" % (
-                len(t), d[0], d[1], d[2], d[3], d[4], d[5], (t[:, 6] - t[:, 0]).mean(), float(first[:, 6].max() - first[:, 0].min())))
     fl = 4.0 * b * H * nq * nk * 64
     print("%-20s fwd %7.1f us (%6.1f TF/s)   bwd %7.1f us (%6.1f TF/s of 3.5x fwd flops)" % (
         name, tf, fl / tf / 1e6, tb, 3.5 * fl / tb / 1e6))

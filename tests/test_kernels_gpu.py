@@ -423,7 +423,7 @@ def test_native_sublayer_executor_equals_python_composition(K, monkeypatch, cros
 
 @pytest.mark.parametrize("nq,nk", [(441, 441), (50, 36), (20, 80), (130, 500)])
 def test_fused_scores_match_unfused_path_and_replay_dropout(K, nq, nk):
-    """bb_attn_scores (softmax / softmax-backward in the tcgen05 epilogue) vs GEMM -> fp32 scores -> softmax kernels:
+    """bb_attn_scores (softmax / softmax-backward on the wgmma accumulators) vs GEMM -> fp32 scores -> softmax kernels:
     same probabilities, identical dropout mask (same counters), same dS and dbias."""
     B, H, dh = 2, 12, 64
     Hd = H * dh
@@ -589,7 +589,7 @@ def test_native_pano_layer_equals_python_composition(K, monkeypatch):
                                               (512, 441, True, 1), (300, 600, True, 1), (36, 36, False, 2), (23, 80, True, 2),
                                               (5, 7, True, 2)])
 def test_tcgen05_attention_forward_matches_fp32_and_mma_sync_paths(K, nq, nk, cross, mode):
-    """csrc/attn_tc.cu (tcgen05 + TMA, S in TMEM) vs fp32 torch attention and vs the mma.sync kernel (same LSE, same
+    """csrc/attn_tc.cu (wgmma + TMA, S in registers) vs fp32 torch attention and vs the mma.sync kernel (same LSE, same
     dropout decisions): key masks (-10000 / -inf, a fully masked sample), ragged tails, 1..3 super-blocks."""
     B, H, Hd = 3, 12, 768
     if not cross:
@@ -667,7 +667,7 @@ def test_project_bev_reference_entry_point_bit_exact(K):
                                               (130, 200, True, 1), (100, 512, True, 1), (512, 441, True, 1),
                                               (36, 36, False, 2), (23, 80, True, 2), (5, 7, True, 2)])
 def test_tcgen05_attention_backward_matches_fp32_autograd(K, nq, nk, cross, mode):
-    """csrc/attn_tc.cu backward (two tcgen05 passes: dQ per query tile, dK/dV per key tile) vs fp32 torch autograd with
+    """csrc/attn_tc.cu backward (two wgmma passes: dQ per query tile, dK/dV per key tile) vs fp32 torch autograd with
     key masks (-10000 / -inf) and ragged tails, outputs written into packed views; plus dropout replay against the
     mma.sync backward on the same forward state."""
     B, H, Hd = 2, 12, 768

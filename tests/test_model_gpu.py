@@ -1,4 +1,4 @@
-"""Model-level parity on the GPU: GlocalTextPathCMTPreTraining on the sm_100a kernels (bf16 activations)
+"""Model-level parity on the GPU: GlocalTextPathCMTPreTraining on the sm_90a kernels (bf16 activations)
 against the fp32 CPU oracle, same seeded weights and synthetic batches; losses, logits and every parameter
 gradient.  Tolerances (north_star): 1e-2 relative for the bf16 path."""
 import os
@@ -246,7 +246,7 @@ def test_wire_format_matches_oracle_and_is_exact_for_labels(task):
 def test_rxr_config_long_instruction_xlmr_vocab(task):
     """BASELINE.json configs[3] at reduced depth / batch: XLM-R vocabulary (250002 rows, tied MLM decoder = a 250k-wide
     vocab GEMM + cross-entropy), 514 positions, 512-token instructions -- the 512-key language self-attention and the
-    512-key / 121-query cross-attention run through the tcgen05 attention kernels (8 key blocks), configs/rxr_model.json:20,30."""
+    512-key / 121-query cross-attention run through the wgmma attention kernels (8 key blocks), configs/rxr_model.json:20,30."""
     cfg = small_config(vocab_size=250002, max_position_embeddings=514)
     scfg = small_synth(txt_len=512, vocab_lo=1000, vocab_hi=250000, n_mask_tokens=40)
     _compare(task, cfg, scfg, seed=5)

@@ -49,4 +49,7 @@ def test_oracle_reproduces_reference_outputs(name):
             assert sd[n].grad is not None, n
             assert abs(float(sd[n].grad.norm()) - gn) <= 1e-3 * max(gn, 1e-4 * top), (task, n)
         for n, gr in g["grads"].items():
-            assert torch.allclose(sd[n].grad, gr, rtol=1e-3, atol=1e-4 * float(gr.abs().max()) + 1e-9), (task, n)
+            # same noise floor as the norms above: a mathematically zero gradient (e.g. a bias that only shifts every
+            # logit of a softmax) is rounding noise whose value depends on the host's BLAS and thread count
+            atol = max(1e-4 * float(gr.abs().max()), 1e-3 * 1e-4 * top) + 1e-9
+            assert torch.allclose(sd[n].grad, gr, rtol=1e-3, atol=atol), (task, n)

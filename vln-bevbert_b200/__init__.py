@@ -1,7 +1,7 @@
-"""bevbert_b200 -- B200-native implementation of BEVBert's hybrid-map cross-modal encoder hot path.
+"""bevbert_b200 -- H100-native implementation of BEVBert's hybrid-map cross-modal encoder hot path.
 
 Layout:
-  csrc/ + libbevbert_b200.so   hand-written sm_100a kernels behind the C ABI (include/bevbert_b200.h)
+  csrc/ + libbevbert_b200.so   hand-written sm_90a kernels behind the C ABI (include/bevbert_b200.h)
   _lib.py                      ctypes loader (fails loudly when the library is missing)
   kernels.py                   one thin tensor-level wrapper per C-ABI entry point
   blocks.py                    forward/backward of the encoder blocks, composed from kernels

@@ -301,6 +301,19 @@ def lin_bwd_dx(dy, w16, epi_mul=K.EPI_NONE, aux_in=None, add_in=None, drop=NO_DR
     return out
 
 
+_SMS = {}
+
+
+def _num_sms(device) -> int:
+    """Streaming multiprocessors of `device`, for host-side tiling heuristics (132, an H100 SXM, off the GPU)."""
+    if device.type != "cuda":
+        return 132
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    if idx not in _SMS:
+        _SMS[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _SMS[idx]
+
+
 def lin_bwd_dw(dy, x, out=None):
     """dW = dy^T @ x in fp32: dy (M,N), x (M,Kd), both read MN-major, split over the token dimension.
     `out` (zero-filled fp32 (N,Kd)) is accumulated into when given."""
@@ -308,15 +321,17 @@ def lin_bwd_dw(dy, x, out=None):
     Kd = x.shape[1]
     if out is None:
         out = zeros_f32(dy.device, N, Kd)
-    # few output tiles (weights are small) but a long reduction over tokens: prefer 128-wide tiles when 256-wide
-    # ones cannot fill half the SMs, then split the token dimension until ~148 CTAs, keeping >= 8 k-blocks per split
+    # few output tiles (weights are small) but a long reduction over tokens: prefer 64-wide tiles when 128-wide
+    # ones cannot fill half the SMs, then split the token dimension until about one CTA per SM, keeping >= 8 k-blocks
+    # per split
+    sms = _num_sms(dy.device)
     m_t = (N + 127) // 128
-    bn = 256 if m_t * ((Kd + 255) // 256) >= 74 else 128
+    bn = 128 if m_t * ((Kd + 127) // 128) >= sms // 2 else 64
     if Kd <= bn:
         bn = 0
     tiles = m_t * ((Kd + max(bn, 1) - 1) // max(bn, 1)) if bn else m_t
     kb = (M + 63) // 64
-    split = max(1, min((148 + tiles // 2) // max(tiles, 1), kb // 8 if kb >= 8 else 1))
+    split = max(1, min((sms + tiles // 2) // max(tiles, 1), kb // 8 if kb >= 8 else 1))
     K.gemm(dy, x, out, N, Kd, M, lda=N, ldb=Kd, ldd=Kd, a_mn=True, b_mn=True, split_k=split, block_n=bn)
     return out
 

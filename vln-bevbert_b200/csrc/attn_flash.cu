@@ -1,14 +1,14 @@
 // Fused attention core for head dim 64: softmax(alpha Q K^T + kmask + bias) V with probability dropout, forward and
 // backward, without ever writing the (nq x nk) score / probability matrices to HBM.
 //
-// Why a separate kernel next to the tcgen05 GEMM: on this path the attention products are tiny per (sample, head)
+// Why a separate kernel next to the wgmma GEMM: on this path the attention products are tiny per (sample, head)
 // problems -- 80x80, 36x36, ~23x23, 23x80, 441x80 and 441x441, all with K = 64 -- 384..2148 of them per launch.  As
 // batched GEMMs they are one k-block per tile, so the unfused sequence (QK^T -> fp32 scores -> softmax kernel -> P ->
 // PV, and five launches in backward) is bound by writing and re-reading the score matrices (0.3 GB per 441-key layer)
 // and by per-launch latency, not by tensor throughput (measured 48 TFLOP/s on the 441x441x64 score GEMM).  Here one CTA
 // owns 64 queries (or 64 keys) of one (sample, head), streams the other side through shared memory in 64-row tiles
 // with cp.async, keeps S / P / dS in registers (warp-level mma.sync m16n8k16 bf16, fp32 accumulate; the tiles are too
-// small for a 128-row tcgen05 instruction to pay) and uses the online-softmax recurrence, so HBM traffic is Q, K, V,
+// small for a 64-row warpgroup instruction to pay) and uses the online-softmax recurrence, so HBM traffic is Q, K, V,
 // O (+ dO, dQ, dK, dV) only.  Backward recomputes P from the saved row log-sum-exp:
 //   kernel A (per 64 queries): D = rowsum(dO * O), dQ = alpha * dS K,            dbias += dS
 //   kernel B (per 64 keys)   : dV = Pdrop^T dO,    dK = alpha * dS^T Q
@@ -605,7 +605,7 @@ extern "C" int bb_flash_fwd(const bb_flash_args* a, void* stream) {
   using namespace bb;
   fa::Params p;
   if (int e = fa::fill(p, a, false)) return e;
-  if (fat::fwd_supported(a)) return fat::launch_fwd(a, stream);   // tcgen05 / TMA core (attn_tc.cu)
+  if (fat::fwd_supported(a)) return fat::launch_fwd(a, stream);   // wgmma / TMA core (attn_tc.cu)
   const dim3 grid((unsigned)((a->nq + fa::BM - 1) / fa::BM), (unsigned)a->H, (unsigned)a->B);
   launch_pdl(fa::flash_fwd_kernel, grid, dim3(fa::NT), 0, (cudaStream_t)stream, p);
   count_launch();
@@ -616,7 +616,7 @@ extern "C" int bb_flash_bwd(const bb_flash_args* a, void* stream) {
   using namespace bb;
   fa::Params p;
   if (int e = fa::fill(p, a, true)) return e;
-  if (fat::bwd_supported(a)) return fat::launch_bwd(a, stream);   // tcgen05 / TMA core (attn_tc.cu)
+  if (fat::bwd_supported(a)) return fat::launch_bwd(a, stream);   // wgmma / TMA core (attn_tc.cu)
   const dim3 gq((unsigned)((a->nq + fa::BM - 1) / fa::BM), (unsigned)a->H, (unsigned)a->B);
   const dim3 gk((unsigned)((a->nk + fa::BM - 1) / fa::BM), (unsigned)a->H, (unsigned)a->B);
   launch_pdl(fa::flash_bwd_dq_kernel, gq, dim3(fa::NT), 0, (cudaStream_t)stream, p);

@@ -1,9 +1,11 @@
-// Fused attention-score kernels for sm_100a (keys per row <= 512, head dim 64):
+// Fused attention-score kernels for sm_90a (keys per row <= 512, head dim 64):
 //   mode 0:  P  = softmax(alpha * Q K^T + kmask + bias)  (+ dropped copy Pd)         -- forward
 //   mode 1:  dS = P o (g - sum_k P g) * out_scale,  g = (dO V^T) o dropout-mask        -- backward
-// The 128 x nk product of one (sample, head, query tile) is formed by tcgen05.mma straight into TMEM
-// (operands by TMA into 128B-swizzled shared memory, double buffered across tiles) and the row-wise softmax /
-// softmax-backward runs in the epilogue warps out of TMEM: the fp32 score matrix never exists in HBM.
+// A CTA owns 128 query rows of one (sample, head); Q and all (<= 512) K rows arrive by TMA in 128B-swizzled shared
+// memory (double buffered across tiles).  Each of the two consumer warpgroups forms its 64 x nk product with wgmma,
+// 64 keys at a time into registers, and runs the row-wise softmax / softmax-backward on the fragments in two passes
+// (statistics, then outputs -- the 64-key block is recomputed, which costs tensor time that is otherwise idle):
+// the fp32 score matrix never exists in HBM.
 // Replaces the (batched GEMM -> fp32 scores -> bb_softmax_fwd/bwd) pair of the unfused path; same dropout
 // counters (row * ld + column), so forward and backward stay interchangeable with the unfused kernels.
 //
@@ -21,15 +23,23 @@
 
 namespace bb {
 
-constexpr int AS_EPI_WARPS = 16;           // 4 warps per TMEM lane quarter, each owning every 4th 16-column chunk
-constexpr int AS_THREADS = 64 + 32 * AS_EPI_WARPS;  // warp 0 TMA, warp 1 MMA, warps 2..17 epilogue
+constexpr int AS_THREADS = 288;            // warps 0..7: two consumer warpgroups (64 query rows each), warp 8: TMA
 constexpr int AS_Q_BYTES = 128 * 64 * 2;   // 16 KB
 constexpr int AS_K_BYTES = 512 * 64 * 2;   // 64 KB
 constexpr int AS_STAGE = AS_Q_BYTES + AS_K_BYTES;
 constexpr int AS_STAGES = 2;
 
+__device__ __forceinline__ float quad_max_f(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum_f(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
 struct ScoreParams {
-  int B, H, nq, nk, ldp, m_tiles, kbox, n_loads, mode;
+  int B, H, nq, nk, ldp, m_tiles, mode;
   float alpha, out_scale, scale;
   unsigned long long seed;
   unsigned int thresh;
@@ -42,6 +52,21 @@ struct ScoreParams {
   float* dbias;
 };
 
+// 64 query rows x 64 keys (block c) of the product into this warpgroup's accumulator fragment
+__device__ __forceinline__ void score_block(float (&s)[32], uint32_t sq, uint32_t sk, int c) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) s[i] = 0.0f;
+  fence_regs(s);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_m64n64_ss<0, 0>(s, wgmma_desc(sq + k * 32, 16, 1024), wgmma_desc(sk + c * 8192 + k * 32, 16, 1024),
+                          k > 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(s);
+}
+
 __global__ void __launch_bounds__(AS_THREADS, 1)
 attn_scores_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                    const ScoreParams p, int total_tiles) {
@@ -49,41 +74,25 @@ attn_scores_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + AS_STAGES * AS_STAGE);
   uint64_t* empty_bar = full_bar + AS_STAGES;
-  uint64_t* tmem_full = empty_bar + AS_STAGES;
-  uint64_t* tmem_empty = tmem_full + 1;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 1);
-  float* skm = reinterpret_cast<float*>(smem + AS_STAGES * AS_STAGE + 256);  // [2][512] key masks
-  float* red_a = skm + 2 * 512;                                              // [4][128] partial max / dot
-  float* red_b = red_a + 4 * 128;                                            // [4][128] partial sum
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < AS_STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);
     }
-    mbar_init(tmem_full, 1);
-    mbar_init(tmem_empty, AS_EPI_WARPS);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
   pdl_trigger();
-  const int ncols = (p.nk + 15) & ~15;  // columns the MMAs produce
+  const int nkb = (p.nk + 63) / 64;     // 64-key blocks of the product
+  const int nkb_out = (p.ldp + 63) / 64;  // 64-column blocks of the output rows (columns >= nk are written as 0)
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -91,221 +100,182 @@ attn_scores_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         const int mt = tile % p.m_tiles;
         const int h = (tile / p.m_tiles) % p.H;
         const int b = tile / (p.m_tiles * p.H);
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_wait_relaxed(&empty_bar[stage], phase ^ 1);
         uint8_t* sq = smem + stage * AS_STAGE;
         uint8_t* sk = sq + AS_Q_BYTES;
-        mbar_expect_tx(&full_bar[stage], AS_Q_BYTES + p.n_loads * p.kbox * 128);
+        mbar_expect_tx(&full_bar[stage], AS_Q_BYTES + nkb * 8192);
         tma_load_4d(sq, &tmap_a, &full_bar[stage], 0, mt * 128, h, b);
-        for (int j = 0; j < p.n_loads; ++j)
-          tma_load_4d(sk + j * p.kbox * 128, &tmap_b, &full_bar[stage], 0, j * p.kbox, h, b);
+        for (int j = 0; j < nkb; ++j) tma_load_4d(sk + j * 8192, &tmap_b, &full_bar[stage], 0, j * 64, h, b);
         if (++stage == AS_STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, tphase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(tmem_empty, tphase ^ 1);
-        tc_fence_after();
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sq = smem_u32(smem + stage * AS_STAGE);
-        const uint32_t sk = sq + AS_Q_BYTES;
-        for (int c0 = 0; c0 < ncols; c0 += 256) {
-          const int n_c = min(256, ncols - c0);
-          const uint32_t idesc = umma_idesc_bf16(128, n_c, 0, 0);
+    return;
+  }
+  // -------------------------------------------------------------------- consumers: row-wise softmax on the fragments
+  // Thread t of warpgroup wg holds query rows r0 = 16 (t / 32) + (t % 32) / 4 and r0 + 8 of the tile's 64-row half and,
+  // of each 64-key block, columns 8 j + 2 (t % 4) + {0, 1}; a row lives in the 4 threads of a quad.
+  const int wg = warp >> 2;
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int mt = tile % p.m_tiles;
+    const int h = (tile / p.m_tiles) % p.H;
+    const int b = tile / (p.m_tiles * p.H);
+    int q[2];
+    bool row_ok[2];
+    long long grow[2];   // global row index of P / dS
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(tmem_base + c0, umma_smem_desc(sq + k * 32, 16, 1024),
-                         umma_smem_desc(sk + c0 * 128 + k * 32, 16, 1024), idesc, k > 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        umma_commit(tmem_full);
-        tphase ^= 1;
-        if (++stage == AS_STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
+    for (int hh = 0; hh < 2; ++hh) {
+      q[hh] = mt * 128 + wg * 64 + r0 + 8 * hh;
+      row_ok[hh] = q[hh] < p.nq;
+      grow[hh] = ((long long)b * p.H + h) * p.nq + q[hh];
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue: row-wise softmax out of TMEM
-    // 16 warps: warp w reads TMEM lanes 32*(w%4)..+31 (one query row per lane) and the 16-column chunks
-    // part, part+4, part+8, ... ; the four parts of a row are combined through shared memory.
-    const int quarter = warp & 3;
-    const int part = (warp - 2) >> 2;     // 0..3
-    const int rl = quarter * 32 + lane;   // row within the tile
-    const int e = (warp - 2) * 32 + lane; // 0..511
-    constexpr int NT = 32 * AS_EPI_WARPS;
-    uint32_t tphase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int mt = tile % p.m_tiles;
-      const int h = (tile / p.m_tiles) % p.H;
-      const int b = tile / (p.m_tiles * p.H);
-      const int q = mt * 128 + rl;
-      const bool row_ok = q < p.nq;
-      const long long grow = ((long long)b * p.H + h) * p.nq + q;  // global row index of P / dS
-      float* km = skm + (it & 1) * 512;
-      if (p.mode == 0) {
-        for (int i = e; i < ncols; i += NT)
-          km[i] = (i < p.nk) ? (p.kmask ? __ldg(p.kmask + (long long)b * p.nk + i) : 0.0f) : -INFINITY;
-      }
-      const float* brow = (p.mode == 0 && p.bias && row_ok) ? p.bias + ((long long)b * p.nq + q) * p.nk : nullptr;
-      const __nv_bfloat16* prow = (p.mode == 1 && row_ok) ? p.Pin + grow * p.ldp : nullptr;
-
-      mbar_wait(tmem_full, tphase);
-      tc_fence_after();
-      asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");  // key masks visible
-      const uint32_t taddr = tmem_base + (uint32_t(quarter * 32) << 16);
-
-      if (p.mode == 0) {
-        // pass A: online row maximum / sum of exponentials over this warp's chunks
-        float mx = -INFINITY, sum = 0.0f;
-        for (int c = part * 16; c < ncols; c += 64) {
-          uint32_t r[16];
-          tmem_ld16(taddr + c, r);
-          tmem_ld_wait();
-          float sv[16];
+    const uint32_t sq = smem_u32(smem + stage * AS_STAGE) + wg * 8192;
+    const uint32_t sk = smem_u32(smem + stage * AS_STAGE) + AS_Q_BYTES;
+    mbar_wait(&full_bar[stage], phase);
+    float s[32];
+    if (p.mode == 0) {
+      // scores with mask and bias, for the 16 columns of block c held by this thread
+      auto scores = [&](int c) {
+        score_block(s, sq, sk, c);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = c * 64 + 8 * jj + cq + e;
+            const float km = col < p.nk ? (p.kmask ? __ldg(p.kmask + (long long)b * p.nk + col) : 0.0f) : -INFINITY;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              float v = fmaf(s[4 * jj + 2 * hh + e], p.alpha, km);
+              if (p.bias && row_ok[hh] && col < p.nk) v += __ldg(p.bias + ((long long)b * p.nq + q[hh]) * p.nk + col);
+              s[4 * jj + 2 * hh + e] = v;
+            }
+          }
+      };
+      // pass A: online row maximum / sum of exponentials
+      float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.0f, 0.0f};
+      for (int c = 0; c < nkb; ++c) {
+        scores(c);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
           float cm = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float s = fmaf(__uint_as_float(r[i]), p.alpha, km[c + i]);
-            if (brow && c + i < p.nk) s += __ldg(brow + c + i);
-            sv[i] = s;
-            cm = fmaxf(cm, s);
+          for (int jj = 0; jj < 8; ++jj) cm = fmaxf(cm, fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
+          if (cm > mx[hh]) {
+            sum[hh] *= __expf(mx[hh] - cm);   // exp(-inf) = 0 on the first block
+            mx[hh] = cm;
           }
-          if (cm > mx) {
-            sum *= __expf(mx - cm);   // exp(-inf) = 0 on the first chunk
-            mx = cm;
+          if (mx[hh] > -INFINITY) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) sum[hh] += __expf(s[4 * jj + 2 * hh] - mx[hh]) + __expf(s[4 * jj + 2 * hh + 1] - mx[hh]);
           }
-          if (mx > -INFINITY) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) sum += __expf(sv[i] - mx);
-          }
-        }
-        red_a[part * 128 + rl] = mx;
-        red_b[part * 128 + rl] = sum;
-        asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
-        float m = fmaxf(fmaxf(red_a[rl], red_a[128 + rl]), fmaxf(red_a[256 + rl], red_a[384 + rl]));
-        float l = 0.0f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float mj = red_a[j * 128 + rl];
-          l += (mj > -INFINITY) ? red_b[j * 128 + rl] * __expf(mj - m) : 0.0f;
-        }
-        const float inv = 1.0f / l;     // all keys masked with -inf: 1/0 -> inf, probabilities NaN like torch
-        // pass B: probabilities (and their dropped copy)
-        for (int c = part * 16; c < p.ldp; c += 64) {
-          uint32_t r[16];
-          tmem_ld16(taddr + c, r);
-          tmem_ld_wait();
-          if (!row_ok) continue;
-          float pr[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float s = fmaf(__uint_as_float(r[i]), p.alpha, km[c + i]);
-            if (brow && c + i < p.nk) s += __ldg(brow + c + i);
-            pr[i] = (c + i < p.nk) ? __expf(s - m) * inv : 0.0f;
-          }
-          const int nvalid = min(16, p.ldp - c);  // ldp is a multiple of 8: 8 or 16
-          __align__(16) __nv_bfloat162 hp[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) hp[i] = __floats2bfloat162_rn(pr[2 * i], pr[2 * i + 1]);
-          uint4* dst = reinterpret_cast<uint4*>(p.P + grow * p.ldp + c);
-          dst[0] = reinterpret_cast<uint4*>(hp)[0];
-          if (nvalid == 16) dst[1] = reinterpret_cast<uint4*>(hp)[1];
-          if (p.Pd) {
-            if (p.thresh) {
-              const uint64_t base = (uint64_t)(grow * p.ldp + c);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) pr[i] = drop_keep(p.seed, base + i, p.thresh) ? pr[i] * p.scale : 0.0f;
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) hp[i] = __floats2bfloat162_rn(pr[2 * i], pr[2 * i + 1]);
-            uint4* dd = reinterpret_cast<uint4*>(p.Pd + grow * p.ldp + c);
-            dd[0] = reinterpret_cast<uint4*>(hp)[0];
-            if (nvalid == 16) dd[1] = reinterpret_cast<uint4*>(hp)[1];
-          }
-        }
-      } else {
-        // backward: dot = sum_k P g ; dS = P (g - dot) * out_scale
-        float dot = 0.0f;
-        for (int c = part * 16; c < ncols; c += 64) {
-          uint32_t r[16];
-          tmem_ld16(taddr + c, r);
-          __align__(16) __nv_bfloat16 hp[16];
-          if (row_ok) {
-            const int nvalid = min(16, p.ldp - c);
-            reinterpret_cast<uint4*>(hp)[0] = __ldg(reinterpret_cast<const uint4*>(prow + c));
-            reinterpret_cast<uint4*>(hp)[1] =
-                nvalid == 16 ? __ldg(reinterpret_cast<const uint4*>(prow + c) + 1) : make_uint4(0, 0, 0, 0);
-          }
-          tmem_ld_wait();
-          if (row_ok) {
-            const uint64_t base = (uint64_t)(grow * p.ldp + c);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              if (c + i < p.nk) {
-                float g = __uint_as_float(r[i]);
-                if (p.thresh) g = drop_keep(p.seed, base + i, p.thresh) ? g * p.scale : 0.0f;
-                dot = fmaf(__bfloat162float(hp[i]), g, dot);
-              }
-            }
-          }
-        }
-        red_a[part * 128 + rl] = dot;
-        asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
-        dot = (red_a[rl] + red_a[128 + rl]) + (red_a[256 + rl] + red_a[384 + rl]);
-        for (int c = part * 16; c < p.ldp; c += 64) {
-          const int nvalid = min(16, p.ldp - c);
-          uint32_t r[16];
-          tmem_ld16(taddr + c, r);
-          __align__(16) __nv_bfloat16 hp[16];
-          if (row_ok) {
-            reinterpret_cast<uint4*>(hp)[0] = __ldg(reinterpret_cast<const uint4*>(prow + c));
-            reinterpret_cast<uint4*>(hp)[1] =
-                nvalid == 16 ? __ldg(reinterpret_cast<const uint4*>(prow + c) + 1) : make_uint4(0, 0, 0, 0);
-          }
-          tmem_ld_wait();
-          if (!row_ok) continue;
-          float ds[16];
-          const uint64_t base = (uint64_t)(grow * p.ldp + c);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float d = 0.0f;
-            if (c + i < p.nk) {
-              float g = __uint_as_float(r[i]);
-              if (p.thresh) g = drop_keep(p.seed, base + i, p.thresh) ? g * p.scale : 0.0f;
-              d = __bfloat162float(hp[i]) * (g - dot);
-              if (p.dbias) atomicAdd(p.dbias + ((long long)b * p.nq + q) * p.nk + c + i, d);
-            }
-            ds[i] = d * p.out_scale;
-          }
-          __align__(16) __nv_bfloat162 ho[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) ho[i] = __floats2bfloat162_rn(ds[2 * i], ds[2 * i + 1]);
-          uint4* dst = reinterpret_cast<uint4*>(p.dS + grow * p.ldp + c);
-          dst[0] = reinterpret_cast<uint4*>(ho)[0];
-          if (nvalid == 16) dst[1] = reinterpret_cast<uint4*>(ho)[1];
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty);
-      tphase ^= 1;
+      float m[2], inv[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        m[hh] = quad_max_f(mx[hh]);
+        const float part = mx[hh] > -INFINITY ? sum[hh] * __expf(mx[hh] - m[hh]) : 0.0f;
+        inv[hh] = 1.0f / quad_sum_f(part);   // all keys masked with -inf: 1/0 -> inf, probabilities NaN like torch
+      }
+      // pass B: probabilities (and their dropped copy)
+      for (int c = 0; c < nkb_out; ++c) {
+        if (c < nkb) scores(c);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = c * 64 + 8 * jj + cq;
+          if (col >= p.ldp) continue;   // ldp is a multiple of 8: both columns of the pair are in the row
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if (!row_ok[hh]) continue;
+            float pr[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) pr[e] = (col + e < p.nk) ? __expf(s[4 * jj + 2 * hh + e] - m[hh]) * inv[hh] : 0.0f;
+            const long long off = grow[hh] * p.ldp + col;
+            *reinterpret_cast<__nv_bfloat162*>(p.P + off) = __floats2bfloat162_rn(pr[0], pr[1]);
+            if (p.Pd) {
+              if (p.thresh) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) pr[e] = drop_keep(p.seed, (uint64_t)(off + e), p.thresh) ? pr[e] * p.scale : 0.0f;
+              }
+              *reinterpret_cast<__nv_bfloat162*>(p.Pd + off) = __floats2bfloat162_rn(pr[0], pr[1]);
+            }
+          }
+        }
+      }
+    } else {
+      // backward: g = (dO V^T) o dropout-mask ; dot = sum_k P g ; dS = P o (g - dot) * out_scale
+      auto grads = [&](int c) {
+        score_block(s, sq, sk, c);
+        if (p.thresh) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const uint64_t idx = (uint64_t)(grow[hh] * p.ldp + c * 64 + 8 * jj + cq + e);
+                float& g = s[4 * jj + 2 * hh + e];
+                g = drop_keep(p.seed, idx, p.thresh) ? g * p.scale : 0.0f;
+              }
+        }
+      };
+      auto pin = [&](int hh, int col) {   // P of (row hh, col .. col + 1); col < ldp
+        return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.Pin + grow[hh] * p.ldp + col));
+      };
+      float dot[2] = {0.0f, 0.0f};
+      for (int c = 0; c < nkb; ++c) {
+        grads(c);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = c * 64 + 8 * jj + cq;
+          if (col >= p.nk) continue;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if (!row_ok[hh]) continue;
+            const float2 pv = pin(hh, col);
+            dot[hh] = fmaf(pv.x, s[4 * jj + 2 * hh], dot[hh]);
+            if (col + 1 < p.nk) dot[hh] = fmaf(pv.y, s[4 * jj + 2 * hh + 1], dot[hh]);
+          }
+        }
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) dot[hh] = quad_sum_f(dot[hh]);
+      for (int c = 0; c < nkb_out; ++c) {
+        if (c < nkb) grads(c);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = c * 64 + 8 * jj + cq;
+          if (col >= p.ldp) continue;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if (!row_ok[hh]) continue;
+            const float2 pv = pin(hh, col);
+            float ds[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float d = 0.0f;
+              if (col + e < p.nk) {
+                d = (e ? pv.y : pv.x) * (s[4 * jj + 2 * hh + e] - dot[hh]);
+                if (p.dbias) atomicAdd(p.dbias + ((long long)b * p.nq + q[hh]) * p.nk + col + e, d);
+              }
+              ds[e] = d * p.out_scale;
+            }
+            *reinterpret_cast<__nv_bfloat162*>(p.dS + grow[hh] * p.ldp + col) = __floats2bfloat162_rn(ds[0], ds[1]);
+          }
+        }
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == AS_STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
   }
 }
 
@@ -363,9 +333,6 @@ extern "C" int bb_attn_scores(const bb_attn_scores_args* a, void* stream_) {
   memset(&p, 0, sizeof(p));
   p.B = a->B; p.H = a->H; p.nq = a->nq; p.nk = a->nk; p.ldp = a->ldp; p.mode = a->mode;
   p.m_tiles = (a->nq + 127) / 128;
-  const int ncols = (a->nk + 15) & ~15;
-  p.kbox = ncols < 256 ? ncols : 256;
-  p.n_loads = (ncols + p.kbox - 1) / p.kbox;
   p.alpha = a->alpha; p.out_scale = a->out_scale; p.scale = a->scale; p.seed = a->seed; p.thresh = a->thresh;
   p.kmask = a->kmask; p.bias = a->bias;
   p.P = reinterpret_cast<__nv_bfloat16*>(a->P);
@@ -376,11 +343,11 @@ extern "C" int bb_attn_scores(const bb_attn_scores_args* a, void* stream_) {
   CUtensorMap ta, tb;
   int e = make_map_rows(&ta, a->A, a->nq, a->H, a->B, a->lda, a->a_s1, a->a_s2, 128);
   if (e) return e;
-  e = make_map_rows(&tb, a->Bm, a->nk, a->H, a->B, a->ldb, a->b_s1, a->b_s2, p.kbox);
+  e = make_map_rows(&tb, a->Bm, a->nk, a->H, a->B, a->ldb, a->b_s1, a->b_s2, 64);
   if (e) return e;
   const long long total = (long long)p.m_tiles * a->H * a->B;
   const int grid = total < num_sms ? (int)total : num_sms;
-  const size_t smem_bytes = (size_t)AS_STAGES * AS_STAGE + 1024 + 256 + (2 * 512 + 8 * 128) * sizeof(float);
+  const size_t smem_bytes = (size_t)AS_STAGES * AS_STAGE + 1024 + 64;
   bb::launch_pdl(attn_scores_kernel, grid, AS_THREADS, smem_bytes, stream, ta, tb, p, (int)total);
   count_launch();
   return check_launch("attn_scores_kernel");

@@ -1,29 +1,18 @@
-// Attention core on tcgen05 tensor cores, fed by TMA, for head dim 64 and >= 64 keys.
+// Attention core on wgmma tensor cores, fed by TMA, for head dim 64 and >= 64 keys.
 //
 //   O = dropout(softmax(alpha Q K^T + kmask)) V        per (sample, head), scores / probabilities never leave the SM
 //
 // Three kernels live here (dispatch at the bottom: launch_fwd / launch_bwd, called from attn_flash.cu):
-//   attn_tc_fwd2_kernel    the DEFAULT forward: K / V stream in 64-key blocks, 256 TMEM columns, two CTAs per SM
-//                          (described at its definition, "forward, streaming");
-//   attn_tc_bwd_kernel<M>  backward, dQ pass (M = 0) and dK / dV pass (M = 1) (described at its definition);
-//   attn_tc_fwd_kernel     the first-generation forward described next; serves rows longer than 4096 keys (the streaming
-//                          kernel stages the whole key mask in shared memory) and BB_ATTN_FWD=1 (A/B measurements: 146 us
-//                          against 89 us at 441 x 441; the reference point of profiles/r02_attention.md).
-//
-// First-generation forward.  One CTA owns 128 queries of one (sample, head):
-//   warp 0 (one elected lane)  TMA producer + MMA issuer:
-//        Q (128 x 64) and all K / V rows of a "super-block" of up to 448 keys arrive by cp.async.bulk.tensor (128-byte
-//        swizzle, zero fill past the last row); S = Q K^T is one or two tcgen05.mma groups (M 128, N <= 256, 4 k-steps)
-//        into TMEM columns [64, 64 + keys); O += P V is issued per 64-key block as soon as the softmax warps publish it.
-//   warps 1..8 (256 threads)   softmax + epilogue: thread = (query row, key half).  Rows are TMEM lanes, so a thread
-//        reads its own score row with tcgen05.ld (32 columns per instruction), no shuffles:  pass 1 row maximum,
-//        pass 2 p = 2^(s - max), row sum, dropout, bf16 P written to shared memory in the K-major 128B-swizzled layout
-//        the second MMA consumes as its A operand (V is its MN-major B operand straight from the TMA tile).
-//        Finally O (TMEM columns [0, 64)) is normalised by the row sum and stored as bf16, and the row log-sum-exp is
-//        saved for backward.
-// The whole key range of a super-block is in TMEM at once (441 BEV cells -> 448 columns), so there is no online-softmax
-// rescaling of O; longer rows (RxR, 512 keys) run as several super-blocks merged in registers.
-// TMEM: 512 columns = O (64) + S (448).  Shared memory: Q 16 KB + K 56 KB + V 56 KB + P 2 x 16 KB.
+//   attn_tc_fwd_kernel     forward: a CTA owns 128 queries of one (sample, head); K / V stream through a ring of
+//                          shared-memory stages in 64-key blocks;
+//   attn_tc_bwd_kernel<M>  backward, dQ pass (M = 0, CTA = 128 queries) and dK / dV pass (M = 1, CTA = 128 keys).
+// Every CTA is two consumer warpgroups (warps 0..7, 64 rows each) and one TMA producer warp (warp 8).  Scores are
+// wgmma accumulators in registers: thread t of a warpgroup holds rows r0 = 16 (t / 32) + (t % 32) / 4 and r0 + 8 and,
+// of every 8-column group, columns 2 (t % 4) and 2 (t % 4) + 1, so a row lives in the four threads of a quad and row
+// reductions are two shuffles.  That fragment, converted to bf16, is exactly the register A operand of the next
+// wgmma (P V, dS K, P^T dO, dS^T Q), so probabilities and score gradients never touch shared memory; the other
+// operand of those products is the K / V / Q / dO tile read MN-major from the same 128B-swizzled TMA tile.
+// The forward keeps a running row maximum (online softmax, O rescaled when it grows).
 //
 // Reference semantics: BertSelfAttention / BertOutAttention (vilmodel.py:103-154, 325-363); same dropout function and
 // log2-domain LSE as csrc/attn_flash.cu (mma.sync path, kept for < 64 keys and for the graph-bias case).
@@ -44,12 +33,11 @@ namespace bb {
 namespace fat {
 
 typedef __nv_bfloat16 bf16;
-constexpr int BM = 128;
-constexpr int KB = 64;           // keys per K / V / P block
-constexpr int MAX_SBK = 448;     // keys per super-block (S columns in TMEM)
-constexpr int NT = 288;          // warp 0 + 8 softmax warps
-constexpr int O_COL = 0, S_COL = 64;
-constexpr int Q_BYTES = BM * 128, BLK_BYTES = KB * 128, P_BYTES = BM * 128;
+constexpr int BM = 128;          // rows per CTA (two warpgroups of 64)
+constexpr int KB = 64;           // keys (forward, MODE 0) or queries (MODE 1) per streamed block
+constexpr int NT = 288;          // 8 consumer warps + 1 producer warp
+constexpr int NST = 3;           // depth of the streamed-block ring
+constexpr int R_BYTES = BM * 128, BLK_BYTES = KB * 128;
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct FwdParams {
@@ -59,23 +47,11 @@ struct FwdParams {
   float* lse;
   const float* kmask;
   int B, H, nq, nk;
-  int nsb, sbk;       // super-blocks, keys per super-block (multiple of 64)
   float a2;           // alpha * log2(e)
   uint64_t seed;
   uint32_t thresh;
   float scale;
-  int tmem_cols;
-  long long* trace;   // debug: 8 %globaltimer stamps per CTA (first 256 CTAs) or null
 };
-__device__ __forceinline__ long long gtimer() {
-  long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define FAT_STAMP(i)                                                                                       \
-  do {                                                                                                     \
-    if (p.trace && st == 0 && cta_lin < 256) p.trace[cta_lin * 8 + (i)] = gtimer();                        \
-  } while (0)
 
 __device__ __forceinline__ float ex2f(float x) {
   float y;
@@ -96,593 +72,194 @@ __device__ __forceinline__ uint32_t mix_pair(uint32_t rowhash, uint32_t pair) {
   x ^= x >> 16;
   return x;
 }
-// explicit shared-space accesses: the carve-up of the dynamic shared memory goes through integer arithmetic, after which
-// the compiler no longer knows the address space and emits generic LD / ST (measured: the top long-scoreboard stalls)
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
+// keep decision of key k (of the pair hash x): the even key of a pair tests the low 16 bits, the odd key the high 16
+__device__ __forceinline__ bool keep_key(uint32_t x, int k, uint32_t t16s) {
+  return (k & 1) ? x >= t16s : (x << 16) >= t16s;
 }
-__device__ __forceinline__ float lds_f(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-__device__ __forceinline__ void sts_f(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-__device__ __forceinline__ void sts_u4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+// accumulator fragment (64 columns) -> bf16 A-operand fragments of the four 16-deep K steps
+__device__ __forceinline__ void to_afrag(const float (&s)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[kk][i] = pack2(s[8 * kk + 2 * i], s[8 * kk + 2 * i + 1]);
 }
-__device__ __forceinline__ void named_sync_256() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// S (+)= A B^T over head dim 64, A and B both K-major 64-row tiles in shared memory
+__device__ __forceinline__ void qk_product(float (&s)[32], uint32_t a, uint32_t b) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_m64n64_ss<0, 0>(s, wgmma_desc(a + k * 32, 16, 1024), wgmma_desc(b + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+}
+// D += P X with P the register fragment (64 rows x 64) and X a [64][64] tile read MN-major
+__device__ __forceinline__ void pv_product(float (&d)[32], const uint32_t (&a)[4][4], uint32_t x) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs<1>(d, a[kk], wgmma_desc(x + kk * 2048, 8192, 1024), 1u);
+}
+__device__ __forceinline__ void store_row_pair(bf16* dst, float v0, float v1) {
+  *reinterpret_cast<uint32_t*>(dst) = pack2(v0, v1);
+}
 
+// ================================================================================================ forward
 __global__ void __launch_bounds__(NT, 1)
 attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                    const __grid_constant__ CUtensorMap tv, const FwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nkb_max = p.sbk / KB;
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Q_BYTES;
-  uint8_t* sV = sK + nkb_max * BLK_BYTES;
-  uint8_t* sP = sV + nkb_max * BLK_BYTES;
-  float* skm = reinterpret_cast<float*>(sP + 2 * P_BYTES);       // [sbk] log2-domain key mask
-  float* smax = skm + p.sbk;                                     // [2][128]
-  float* ssum = smax + 2 * BM;                                   // [2][128]
-  int* skf = reinterpret_cast<int*>(ssum + 2 * BM);              // [16] per 32-key chunk: mask not identically zero
-  uint64_t* bars = reinterpret_cast<uint64_t*>(skf + 16);
-  uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;
-  uint64_t* v_full = bars + 2;
-  uint64_t* s_full = bars + 3;
-  uint64_t* o_full = bars + 4;
-  uint64_t* o_read = bars + 5;
-  uint64_t* p_full = bars + 6;    // [2]
-  uint64_t* p_empty = bars + 8;   // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 10);
+  uint8_t* sK = sQ + R_BYTES;
+  uint8_t* sV = sK + NST * BLK_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + NST * BLK_BYTES);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;          // [NST]
+  uint64_t* kv_free = bars + 1 + NST;    // [NST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * BM, h = blockIdx.y, b = blockIdx.z;
-  const int cta_lin = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-  if (p.trace && threadIdx.x == 32 && cta_lin < 256) p.trace[cta_lin * 8 + 0] = gtimer();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tq);
-      tma_prefetch_desc(&tk);
-      tma_prefetch_desc(&tv);
-      mbar_init(q_full, 1);
-      mbar_init(k_full, 1);
-      mbar_init(v_full, 1);
-      mbar_init(s_full, 1);
-      mbar_init(o_full, 1);
-      mbar_init(o_read, 256);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&p_full[i], 128);
-        mbar_init(&p_empty[i], 1);
-      }
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_ptr_smem, (uint32_t)p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();
-  pdl_trigger();
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer + MMA issuer
-    if (lane == 0) {
-      mbar_expect_tx(q_full, Q_BYTES);
-      tma_load_4d(sQ, &tq, q_full, 0, q0, h, b);
-      const uint32_t idesc_pv = umma_idesc_bf16(BM, 64, 0, 1);
-      uint32_t pf_phase[2] = {0, 0};
-      for (int sb = 0; sb < p.nsb; ++sb) {
-        const int key0 = sb * p.sbk;
-        const int nkeys = min(p.sbk, p.nk - key0);
-        const int nblk = (nkeys + KB - 1) / KB;
-        if (sb > 0) mbar_wait(o_read, (sb - 1) & 1);   // S and O of the previous super-block have been consumed
-        mbar_expect_tx(k_full, nblk * BLK_BYTES);
-        for (int j = 0; j < nblk; ++j) tma_load_4d(sK + j * BLK_BYTES, &tk, k_full, 0, key0 + j * KB, h, b);
-        mbar_expect_tx(v_full, nblk * BLK_BYTES);
-        for (int j = 0; j < nblk; ++j) tma_load_4d(sV + j * BLK_BYTES, &tv, v_full, 0, key0 + j * KB, h, b);
-        if (sb == 0) mbar_wait(q_full, 0);
-        mbar_wait(k_full, sb & 1);
-        tc_fence_after();
-        // S = Q K^T
-        const int n_eff = (nkeys + 31) & ~31;   // whole 32-column chunks are read back; K rows past nk are zero-filled
-        const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK);
-        for (int n0 = 0; n0 < n_eff; n0 += 256) {
-          const int nn = min(256, n_eff - n0);
-          const uint32_t idesc = umma_idesc_bf16(BM, nn, 0, 0);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(tmem_base + S_COL + n0, umma_smem_desc(aQ + k * 32, 16, 1024),
-                         umma_smem_desc(aK + n0 * 128 + k * 32, 16, 1024), idesc, k > 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        // O (+)= P V, one 64-key block at a time
-        mbar_wait(v_full, sb & 1);
-        const uint32_t aP = smem_u32(sP), aV = smem_u32(sV);
-        for (int j = 0; j < nblk; ++j) {
-          const int slot = j & 1;
-          mbar_wait(&p_full[slot], pf_phase[slot]);
-          pf_phase[slot] ^= 1;
-          tc_fence_after();
-          const int ksteps = (min(KB, nkeys - j * KB) + 15) >> 4;
-          for (int k = 0; k < ksteps; ++k)
-            umma_bf16_ss(tmem_base + O_COL, umma_smem_desc(aP + slot * P_BYTES + k * 32, 16, 1024),
-                         umma_smem_desc(aV + j * BLK_BYTES + k * 2048, 8192, 1024), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&p_empty[slot]);
-        }
-        umma_commit(o_full);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------------ softmax + epilogue (256 threads)
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int hf = (warp - 1) >> 2;           // key half: blocks j = hf, hf + 2, ...
-    const int row = quarter * 32 + lane;      // query row in the tile = TMEM lane
-    const int st = threadIdx.x - 32;          // 0..255
-    const uint32_t trow = tmem_base + (uint32_t(quarter * 32) << 16);
-    const int64_t grow = ((int64_t)b * p.H + h) * p.nq + q0 + row;
-    const uint32_t rh = p.thresh ? rng_u32(p.seed, (uint64_t)grow) : 0u;
-    const uint32_t t16s = p.thresh & 0xFFFF0000u;   // keep iff the 16-bit half >= thresh >> 16, compared in the high half
-    const uint32_t prow = smem_u32(sP) + hf * P_BYTES + (row >> 3) * 1024 + (row & 7) * 128;
-    const int sw = row & 7;
-    const uint32_t a_skm = smem_u32(skm), a_smax = smem_u32(smax), a_ssum = smem_u32(ssum), a_skf = smem_u32(skf);
-    uint32_t pe_phase = 0;
-    float m_run = -INFINITY, l_run = 0.f;
-    float o_run[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o_run[i] = 0.f;
-
-    for (int sb = 0; sb < p.nsb; ++sb) {
-      const int key0 = sb * p.sbk;
-      const int nkeys = min(p.sbk, p.nk - key0);
-      const int nblk = (nkeys + KB - 1) / KB;
-      // log2-domain additive key mask of this super-block (previous one fully consumed: o_read / s_full ordering)
-      for (int i = st; i < p.sbk; i += 256) {      // a warp covers exactly one 32-key chunk per iteration
-        const int col = key0 + i;
-        const float kv = i < nkeys ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + col) * LOG2E : 0.f) : -INFINITY;
-        sts_f(a_skm + i * 4, kv);
-        const bool any = __any_sync(0xffffffffu, kv != 0.f);
-        if (lane == 0) sts_f(a_skf + (i >> 5) * 4, any ? 1.f : 0.f);
-      }
-      named_sync_256();
-      FAT_STAMP(1);
-      mbar_wait(s_full, sb & 1);
-      tc_fence_after();
-      FAT_STAMP(2);
-      // ---- pass 1: row maximum over this thread's blocks (chunks without a mask: max of the raw scores, scaled once)
-      float mx = -INFINITY, mraw = -INFINITY;
-      for (int j = hf; j < nblk; j += 2) {
-#pragma unroll
-        for (int c = 0; c < KB; c += 32) {
-          if (j * KB + c < nkeys) {
-            uint32_t r[32];
-            tmem_ld32(trow + S_COL + j * KB + c, r);
-            tmem_ld_wait32(r);
-            if (lds_f(a_skf + ((j * KB + c) >> 5) * 4) == 0.f) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) mraw = fmaxf(mraw, fmaxf(__uint_as_float(r[i]), __uint_as_float(r[i + 1])));
-            } else {
-              const uint32_t km4 = a_skm + (j * KB + c) * 4;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 km = lds_f4(km4 + i * 16);
-                mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * i + 0]), p.a2, km.x));
-                mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * i + 1]), p.a2, km.y));
-                mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * i + 2]), p.a2, km.z));
-                mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * i + 3]), p.a2, km.w));
-              }
-            }
-          }
-        }
-      }
-      mx = fmaxf(mx, mraw * p.a2);      // a2 > 0 (checked on the host)
-      sts_f(a_smax + (hf * BM + row) * 4, mx);
-      named_sync_256();
-      FAT_STAMP(3);
-      const float m = fmaxf(lds_f(a_smax + row * 4), lds_f(a_smax + (BM + row) * 4));
-      const float ms = m == -INFINITY ? 0.f : m;
-      // ---- pass 2: probabilities -> bf16 P blocks in shared memory (A operand of the PV product)
-      float lsum = 0.f;
-      for (int j = hf; j < nblk; j += 2) {
-        mbar_wait(&p_empty[hf], pe_phase ^ 1);
-#pragma unroll
-        for (int c = 0; c < KB; c += 32) {
-          uint32_t pk[16];
-          if (j * KB + c < nkeys) {
-            uint32_t r[32];
-            tmem_ld32(trow + S_COL + j * KB + c, r);
-            tmem_ld_wait32(r);
-            const bool masked = lds_f(a_skf + ((j * KB + c) >> 5) * 4) != 0.f;
-            const uint32_t km4 = a_skm + (j * KB + c) * 4;
-            const uint32_t pair0 = (uint32_t)(key0 + j * KB + c) >> 1;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float e0, e1, e2, e3;
-              if (masked) {
-                const float4 km = lds_f4(km4 + i * 16);
-                e0 = ex2f(fmaf(__uint_as_float(r[4 * i + 0]), p.a2, km.x - ms));
-                e1 = ex2f(fmaf(__uint_as_float(r[4 * i + 1]), p.a2, km.y - ms));
-                e2 = ex2f(fmaf(__uint_as_float(r[4 * i + 2]), p.a2, km.z - ms));
-                e3 = ex2f(fmaf(__uint_as_float(r[4 * i + 3]), p.a2, km.w - ms));
-              } else {
-                e0 = ex2f(fmaf(__uint_as_float(r[4 * i + 0]), p.a2, -ms));
-                e1 = ex2f(fmaf(__uint_as_float(r[4 * i + 1]), p.a2, -ms));
-                e2 = ex2f(fmaf(__uint_as_float(r[4 * i + 2]), p.a2, -ms));
-                e3 = ex2f(fmaf(__uint_as_float(r[4 * i + 3]), p.a2, -ms));
-              }
-              lsum += (e0 + e1) + (e2 + e3);
-              if (p.thresh) {     // kept probabilities are NOT rescaled here: 1/(1-p) is folded into the O epilogue
-                const uint32_t x0 = mix_pair(rh, pair0 + 2 * i), x1 = mix_pair(rh, pair0 + 2 * i + 1);
-                e0 = (x0 << 16) >= t16s ? e0 : 0.f;
-                e1 = x0 >= t16s ? e1 : 0.f;
-                e2 = (x1 << 16) >= t16s ? e2 : 0.f;
-                e3 = x1 >= t16s ? e3 : 0.f;
-              }
-              pk[2 * i] = pack2(e0, e1);
-              pk[2 * i + 1] = pack2(e2, e3);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) pk[i] = 0u;
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {   // 16-byte chunk (c/8 + i) of this row, XOR-swizzled by the row (128B swizzle)
-            const int ch = (c >> 3) + i;
-            sts_u4(prow + ((ch ^ sw) << 4), pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
-          }
-        }
-        fence_proxy_async();          // generic-proxy stores -> visible to the tensor core's async-proxy reads
-        mbar_arrive(&p_full[hf]);
-        pe_phase ^= 1;
-      }
-      sts_f(a_ssum + (hf * BM + row) * 4, lsum);
-      named_sync_256();
-      FAT_STAMP(4);
-      const float l = lds_f(a_ssum + row * 4) + lds_f(a_ssum + (BM + row) * 4);
-      // ---- O of this super-block: columns [32 hf, 32 hf + 32) of the row
-      mbar_wait(o_full, sb & 1);
-      tc_fence_after();
-      FAT_STAMP(5);
-      uint32_t r[32];
-      tmem_ld32(trow + O_COL + hf * 32, r);
-      tmem_ld_wait32(r);
-      const float m_new = fmaxf(m_run, m);
-      const float mb = m_new == -INFINITY ? 0.f : m_new;
-      const float c_run = ex2f(m_run - mb), c_sb = ex2f(m - mb);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o_run[i] = o_run[i] * c_run + __uint_as_float(r[i]) * c_sb;
-      l_run = l_run * c_run + l * c_sb;
-      m_run = m_new;
-      if (sb + 1 < p.nsb) {
-        tc_fence_before();
-        mbar_arrive(o_read);
-      }
-    }
-    // ---- epilogue: normalise, store bf16 rows and the log2-domain log-sum-exp
-    if (q0 + row < p.nq) {
-      const float inv = l_run > 0.f ? (p.thresh ? p.scale : 1.0f) / l_run : 0.f;
-      bf16* dst = p.out + (int64_t)b * p.o_bs + (int64_t)(q0 + row) * p.ldo + h * 64 + hf * 32;
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        reinterpret_cast<uint4*>(dst)[i] = make_uint4(pack2(o_run[8 * i] * inv, o_run[8 * i + 1] * inv),
-                                                      pack2(o_run[8 * i + 2] * inv, o_run[8 * i + 3] * inv),
-                                                      pack2(o_run[8 * i + 4] * inv, o_run[8 * i + 5] * inv),
-                                                      pack2(o_run[8 * i + 6] * inv, o_run[8 * i + 7] * inv));
-      if (hf == 0 && p.lse) p.lse[grow] = l_run > 0.f ? m_run + log2f(l_run) : INFINITY;
-    }
-    FAT_STAMP(6);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
-}
-
-
-// ================================================================================================ forward, streaming
-// Second-generation forward (the default): K / V stream through shared memory in 64-key blocks, S is double-buffered in
-// TMEM (2 x 64 columns + 64 for O = 256 allocated columns) and the CTA is small (10 warps, 98 KB of shared memory), so
-// TWO CTAs share an SM and each one overlaps its own tensor-pipe work with its element-wise work: profiling of the
-// first version (whole key range in TMEM, one CTA per SM) showed 28 % issue utilisation -- the warps mostly waited on
-// mbarriers (loads, MMAs) with nothing else resident to run.
-//   pass A: for every key block  S = Q K^T -> running row maximum                     (tensor pipe + 1 FMNMX / element)
-//   pass B: for every key block  S = Q K^T again -> P = 2^(S - max) -> O += P V       (K is re-streamed from L2)
-// A thread owns a complete query row (TMEM lane), so max and sum need no exchange between warps; recomputing S costs
-// tensor time that is idle anyway (a 128 x 64 x 64 product is 128 cycles) and removes the online-softmax rescaling of O.
-constexpr int F2_NT = 320;                 // warp 0 TMA, warp 1 MMA, warps 2..9 softmax / epilogue (row x key half)
-constexpr int F2_O = 0, F2_S = 64;         // TMEM columns: O [0,64), S buffers [64,128) and [128,192)
-constexpr int F2_KST = 3;                  // K / V ring depth
-
-__device__ __forceinline__ void named_sync_128() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-
-__global__ void __launch_bounds__(F2_NT, 2)
-attn_tc_fwd2_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
-                    const __grid_constant__ CUtensorMap tv, const FwdParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Q_BYTES;
-  uint8_t* sV = sK + F2_KST * BLK_BYTES;
-  uint8_t* sP = sV + F2_KST * BLK_BYTES;
   const int nblk = (p.nk + KB - 1) / KB;
-  const bool keep_s = nblk <= 2;     // both S blocks fit the two TMEM buffers: pass B re-reads them instead of recomputing
-  const int n_s = keep_s ? nblk : 2 * nblk;
-  float* skm = reinterpret_cast<float*>(sP + 2 * P_BYTES);        // [nblk * 64] log2-domain key mask
-  float* skf = skm + nblk * KB;                                   // [nblk * 2] per 32-key chunk: mask not all zero
-  float* sx = skf + ((nblk * 2 + 3) & ~3);                        // [2][128] row max / row sum exchange between halves
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sx + 2 * BM);
-  uint64_t* q_full = bars + 0;
-  uint64_t* o_full = bars + 1;
-  uint64_t* k_full = bars + 2;     // [3]
-  uint64_t* k_free = bars + 5;     // [3]
-  uint64_t* v_full = bars + 8;     // [3]
-  uint64_t* v_free = bars + 11;    // [3]
-  uint64_t* s_full = bars + 14;    // [2]
-  uint64_t* s_free = bars + 16;    // [2]
-  uint64_t* p_full = bars + 18;    // [2]
-  uint64_t* p_free = bars + 20;    // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 22);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * BM, h = blockIdx.y, b = blockIdx.z;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tq);
-      tma_prefetch_desc(&tk);
-      tma_prefetch_desc(&tv);
-      mbar_init(q_full, 1);
-      mbar_init(o_full, 1);
-      for (int i = 0; i < F2_KST; ++i) {
-        mbar_init(&k_full[i], 1);
-        mbar_init(&k_free[i], 1);
-        mbar_init(&v_full[i], 1);
-        mbar_init(&v_free[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&s_free[i], 256);
-        mbar_init(&p_full[i], 256);
-        mbar_init(&p_free[i], 1);
-      }
-      fence_mbar_init();
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tq);
+    tma_prefetch_desc(&tk);
+    tma_prefetch_desc(&tv);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < NST; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_free[i], 8);
     }
-    __syncwarp();
-    tmem_alloc(tmem_ptr_smem, 256);
-    tmem_relinquish();
+    fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer: Q, K (pass A), K + V (pass B)
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      mbar_expect_tx(q_full, Q_BYTES);
+      mbar_expect_tx(q_full, R_BYTES);
       tma_load_4d(sQ, &tq, q_full, 0, q0, h, b);
-      for (int i = 0; i < n_s; ++i) {
-        const int j = i < nblk ? i : i - nblk;
-        const int st = i % F2_KST;
-        mbar_wait_relaxed(&k_free[st], ((i / F2_KST) & 1) ^ 1);
-        mbar_expect_tx(&k_full[st], BLK_BYTES);
-        tma_load_4d(sK + st * BLK_BYTES, &tk, &k_full[st], 0, j * KB, h, b);
-        if (keep_s || i >= nblk) {
-          const int vs = j % F2_KST;
-          mbar_wait_relaxed(&v_free[vs], ((j / F2_KST) & 1) ^ 1);
-          mbar_expect_tx(&v_full[vs], BLK_BYTES);
-          tma_load_4d(sV + vs * BLK_BYTES, &tv, &v_full[vs], 0, j * KB, h, b);
-        }
+      for (int j = 0; j < nblk; ++j) {
+        const int st = j % NST;
+        mbar_wait_relaxed(&kv_free[st], ((j / NST) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[st], 2 * BLK_BYTES);
+        tma_load_4d(sK + st * BLK_BYTES, &tk, &kv_full[st], 0, j * KB, h, b);
+        tma_load_4d(sV + st * BLK_BYTES, &tv, &kv_full[st], 0, j * KB, h, b);
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc_s = umma_idesc_bf16(BM, KB, 0, 0), idesc_pv = umma_idesc_bf16(BM, 64, 0, 1);
-      const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP);
-      mbar_wait_relaxed(q_full, 0);
-      auto issue_pv = [&](int j) {
-        const int slot = j & 1, vs = j % F2_KST;
-        mbar_wait_relaxed(&p_full[slot], (j >> 1) & 1);
-        mbar_wait_relaxed(&v_full[vs], (j / F2_KST) & 1);
-        tc_fence_after();
-        const int ksteps = (min(KB, p.nk - j * KB) + 15) >> 4;
-        for (int k = 0; k < ksteps; ++k)
-          umma_bf16_ss(tmem_base + F2_O, umma_smem_desc(aP + slot * P_BYTES + k * 32, 16, 1024),
-                       umma_smem_desc(aV + vs * BLK_BYTES + k * 2048, 8192, 1024), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&p_free[slot]);
-        umma_commit(&v_free[vs]);
-      };
-      for (int i = 0; i < n_s; ++i) {
-        const int st = i % F2_KST, sb = i & 1;
-        mbar_wait_relaxed(&k_full[st], (i / F2_KST) & 1);
-        if (!keep_s) mbar_wait_relaxed(&s_free[sb], ((i >> 1) & 1) ^ 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_ss(tmem_base + F2_S + sb * KB, umma_smem_desc(aQ + k * 32, 16, 1024),
-                       umma_smem_desc(aK + st * BLK_BYTES + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[sb]);
-        umma_commit(&k_free[st]);
-        if (!keep_s && i > nblk) issue_pv(i - nblk - 1);   // one block of look-ahead: S(j+1) runs while P(j) is produced
-      }
-      if (keep_s) {
-        for (int j = 0; j + 1 < nblk; ++j) issue_pv(j);
-      }
-      issue_pv(nblk - 1);
-      umma_commit(o_full);
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------------ softmax + epilogue: thread = (query row, key half)
-    const int quarter = warp & 3;
-    const int hf = (warp - 2) >> 2;              // columns [32 hf, 32 hf + 32) of every 64-key block
-    const int row = quarter * 32 + lane;
-    const int st_ = threadIdx.x - 64;            // 0..255
-    const uint32_t trow = tmem_base + (uint32_t(quarter * 32) << 16);
-    const int64_t grow = ((int64_t)b * p.H + h) * p.nq + q0 + row;
-    const uint32_t rh = p.thresh ? rng_u32(p.seed, (uint64_t)grow) : 0u;
-    const uint32_t t16s = p.thresh & 0xFFFF0000u;
-    const uint32_t a_skm = smem_u32(skm), a_skf = smem_u32(skf), a_sx = smem_u32(sx);
-    const uint32_t prow0 = smem_u32(sP) + (row >> 3) * 1024 + (row & 7) * 128;
-    const int sw = row & 7;
-    for (int i = st_; i < nblk * KB; i += 256) {      // a warp covers exactly one 32-key chunk per iteration
-      const float kv = i < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + i) * LOG2E : 0.f) : -INFINITY;
-      sts_f(a_skm + i * 4, kv);
-      const bool any = __any_sync(0xffffffffu, kv != 0.f);
-      if (lane == 0) sts_f(a_skf + (i >> 5) * 4, any ? 1.f : 0.f);
-    }
-    named_sync_256();
-    // ---- pass A: row maximum over this thread's half of every block
-    float mx = -INFINITY, mraw = -INFINITY;
-    for (int i = 0; i < nblk; ++i) {
-      const int sb = i & 1;
-      mbar_wait(&s_full[sb], (i >> 1) & 1);
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld32(trow + F2_S + sb * KB + hf * 32, r);
-      tmem_ld_wait32(r);
-      if (!keep_s) {
-        tc_fence_before();
-        mbar_arrive(&s_free[sb]);
-      }
-      if (lds_f(a_skf + (i * 2 + hf) * 4) == 0.f) {
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) mraw = fmaxf(mraw, fmaxf(__uint_as_float(r[e]), __uint_as_float(r[e + 1])));
-      } else {
-        const uint32_t km4 = a_skm + (i * KB + hf * 32) * 4;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float4 km = lds_f4(km4 + e * 16);
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * e + 0]), p.a2, km.x));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * e + 1]), p.a2, km.y));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * e + 2]), p.a2, km.z));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[4 * e + 3]), p.a2, km.w));
-        }
-      }
-    }
-    sts_f(a_sx + (hf * BM + row) * 4, fmaxf(mx, mraw * p.a2));      // a2 > 0
-    named_sync_256();
-    const float m = fmaxf(lds_f(a_sx + row * 4), lds_f(a_sx + (BM + row) * 4));
-    const float ms = m == -INFINITY ? 0.f : m;
-    named_sync_256();                                                // sx is reused for the row sums below
-    // ---- pass B: probabilities -> P blocks (A operand of the PV product)
-    float lsum = 0.f;
-    for (int j = 0; j < nblk; ++j) {
-      const int i = keep_s ? j : nblk + j, sb = i & 1, slot = j & 1;
-      if (!keep_s) {
-        mbar_wait(&s_full[sb], (i >> 1) & 1);
-        tc_fence_after();
-      }
-      uint32_t r[32];
-      tmem_ld32(trow + F2_S + sb * KB + hf * 32, r);
-      tmem_ld_wait32(r);
-      if (!keep_s) {
-        tc_fence_before();
-        mbar_arrive(&s_free[sb]);                 // the next S block is computed while this one is exponentiated
-      }
-      mbar_wait(&p_free[slot], ((j >> 1) & 1) ^ 1);
-      const uint32_t prow = prow0 + slot * P_BYTES;
-      const bool masked = lds_f(a_skf + (j * 2 + hf) * 4) != 0.f;
-      const uint32_t km4 = a_skm + (j * KB + hf * 32) * 4;
-      const uint32_t pair0 = (uint32_t)(j * KB + hf * 32) >> 1;
-#pragma unroll
-      for (int e = 0; e < 8; e += 2) {
-        uint32_t w[4];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int x = e + u;
-          float e0, e1, e2, e3;
-          if (masked) {
-            const float4 km = lds_f4(km4 + x * 16);
-            e0 = ex2f(fmaf(__uint_as_float(r[4 * x + 0]), p.a2, km.x - ms));
-            e1 = ex2f(fmaf(__uint_as_float(r[4 * x + 1]), p.a2, km.y - ms));
-            e2 = ex2f(fmaf(__uint_as_float(r[4 * x + 2]), p.a2, km.z - ms));
-            e3 = ex2f(fmaf(__uint_as_float(r[4 * x + 3]), p.a2, km.w - ms));
-          } else {
-            e0 = ex2f(fmaf(__uint_as_float(r[4 * x + 0]), p.a2, -ms));
-            e1 = ex2f(fmaf(__uint_as_float(r[4 * x + 1]), p.a2, -ms));
-            e2 = ex2f(fmaf(__uint_as_float(r[4 * x + 2]), p.a2, -ms));
-            e3 = ex2f(fmaf(__uint_as_float(r[4 * x + 3]), p.a2, -ms));
-          }
-          lsum += (e0 + e1) + (e2 + e3);
-          if (p.thresh) {     // kept probabilities are not rescaled here: 1/(1-p) is folded into the O epilogue
-            const uint32_t x0 = mix_pair(rh, pair0 + 2 * x), x1 = mix_pair(rh, pair0 + 2 * x + 1);
-            e0 = (x0 << 16) >= t16s ? e0 : 0.f;
-            e1 = x0 >= t16s ? e1 : 0.f;
-            e2 = (x1 << 16) >= t16s ? e2 : 0.f;
-            e3 = x1 >= t16s ? e3 : 0.f;
-          }
-          w[2 * u] = pack2(e0, e1);
-          w[2 * u + 1] = pack2(e2, e3);
-        }
-        sts_u4(prow + (((hf * 4 + (e >> 1)) ^ sw) << 4), w[0], w[1], w[2], w[3]);
-      }
-      fence_proxy_async();
-      mbar_arrive(&p_full[slot]);
-    }
-    sts_f(a_sx + (hf * BM + row) * 4, lsum);
-    named_sync_256();
-    const float l = lds_f(a_sx + row * 4) + lds_f(a_sx + (BM + row) * 4);
-    // ---- epilogue: this thread's 32 columns of the O row -> bf16, log2-domain log-sum-exp
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const float inv = l > 0.f ? (p.thresh ? p.scale : 1.0f) / l : 0.f;
-    const bool valid = q0 + row < p.nq;
-    {
-      uint32_t r[32];
-      tmem_ld32(trow + F2_O + hf * 32, r);
-      tmem_ld_wait32(r);
-      if (valid) {
-        bf16* dst = p.out + (int64_t)b * p.o_bs + (int64_t)(q0 + row) * p.ldo + h * 64 + hf * 32;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          reinterpret_cast<uint4*>(dst)[i] =
-              make_uint4(pack2(__uint_as_float(r[8 * i]) * inv, __uint_as_float(r[8 * i + 1]) * inv),
-                         pack2(__uint_as_float(r[8 * i + 2]) * inv, __uint_as_float(r[8 * i + 3]) * inv),
-                         pack2(__uint_as_float(r[8 * i + 4]) * inv, __uint_as_float(r[8 * i + 5]) * inv),
-                         pack2(__uint_as_float(r[8 * i + 6]) * inv, __uint_as_float(r[8 * i + 7]) * inv));
-      }
-    }
-    if (valid && hf == 0 && p.lse) p.lse[grow] = l > 0.f ? m + log2f(l) : INFINITY;
+    return;
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+  // -------------------------------------------------------------------- consumers (softmax + epilogue)
+  const int wg = warp >> 2;
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t t16s = p.thresh & 0xFFFF0000u;
+  int q[2];
+  uint32_t rh[2];
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    q[hh] = q0 + wg * 64 + r0 + 8 * hh;
+    rh[hh] = p.thresh ? rng_u32(p.seed, (uint64_t)(((int64_t)b * p.H + h) * p.nq + q[hh])) : 0u;
+  }
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  const uint32_t aQ = smem_u32(sQ) + wg * 8192;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % NST;
+    float km[16];   // log2-domain key mask of this thread's 16 columns
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = j * KB + 8 * jj + cq + e;
+        km[2 * jj + e] = c < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + c) * LOG2E : 0.f) : -INFINITY;
+      }
+    mbar_wait(&kv_full[st], (j / NST) & 1);
+    float s[32];
+    fence_regs(s);
+    wgmma_fence();
+    qk_product(s, aQ, smem_u32(sK + st * BLK_BYTES));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float& v = s[4 * jj + i];
+        v = fmaf(v, p.a2, km[2 * jj + (i & 1)]);
+        mx[i >> 1] = fmaxf(mx[i >> 1], v);
+      }
+    float ms[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float mn = fmaxf(m[hh], quad_max(mx[hh]));
+      ms[hh] = mn == -INFINITY ? 0.f : mn;
+      const float corr = ex2f(m[hh] - ms[hh]);
+      m[hh] = mn;
+      l[hh] *= corr;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj + 2 * hh] *= corr;
+        o[4 * jj + 2 * hh + 1] *= corr;
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int c = j * KB + 8 * jj + cq;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float e0 = ex2f(s[4 * jj + 2 * hh] - ms[hh]), e1 = ex2f(s[4 * jj + 2 * hh + 1] - ms[hh]);
+        l[hh] += e0 + e1;
+        if (p.thresh) {     // kept probabilities are NOT rescaled here: 1/(1-p) is folded into the O epilogue
+          const uint32_t x = mix_pair(rh[hh], (uint32_t)c >> 1);
+          e0 = keep_key(x, c, t16s) ? e0 : 0.f;
+          e1 = keep_key(x, c + 1, t16s) ? e1 : 0.f;
+        }
+        s[4 * jj + 2 * hh] = e0;
+        s[4 * jj + 2 * hh + 1] = e1;
+      }
+    }
+    uint32_t a[4][4];
+    to_afrag(s, a);
+    fence_regs(o);
+    wgmma_fence();
+    pv_product(o, a, smem_u32(sV + st * BLK_BYTES));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    if (lane == 0) mbar_arrive(&kv_free[st]);
+  }
+  // ---- epilogue: normalise, store bf16 rows and the log2-domain log-sum-exp
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const float lt = quad_sum(l[hh]);
+    if (q[hh] >= p.nq) continue;
+    const float inv = lt > 0.f ? (p.thresh ? p.scale : 1.0f) / lt : 0.f;
+    bf16* dst = p.out + (int64_t)b * p.o_bs + (int64_t)q[hh] * p.ldo + h * 64 + cq;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) store_row_pair(dst + 8 * jj, o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+    if ((lane & 3) == 0 && p.lse)
+      p.lse[((int64_t)b * p.H + h) * p.nq + q[hh]] = lt > 0.f ? m[hh] + log2f(lt) : INFINITY;
   }
 }
 
 // ================================================================================================ backward
-// Two passes over the (query tile x key tile) grid of a (sample, head), both with 128 x 128 score tiles in TMEM and the
-// thread <-> query-row mapping of the forward kernel:
-//   MODE 0 (CTA = 128 queries): D = rowsum(dO o O);  for each key tile: S = Q K^T, dP = dO V^T  ->  dS  ->  dQ += dS K
-//   MODE 1 (CTA = 128 keys)   : for each query tile: S = Q K^T, dP = dO V^T -> Pdrop, dS -> dV += Pdrop^T dO, dK += dS^T Q
-// with P = 2^(a2 S + kmask - lse), dS = alpha P o (drop(dP) - D).  S and dP are two tcgen05.mma groups into TMEM columns
-// [0,128) and [128,256); the softmax warps turn them into bf16 Pdrop / dS tiles in shared memory ([query][key], 128B
-// swizzle), which the second round of MMAs reads as a K-major A operand (dS K) or as an MN-major A operand (P^T dO,
-// dS^T Q); accumulators (dQ, or dV and dK) live in TMEM columns [256,384) for the whole CTA.  No atomics.
-constexpr int B_S_COL = 0, B_DP_COL = 128, B_ACC0 = 256, B_ACC1 = 320;
-constexpr int TILE_BYTES = 128 * 128;    // 128 rows x 64 bf16
-
+// Two passes over the (query x key) grid of a (sample, head), both with P = 2^(a2 S + kmask - lse) recomputed from the
+// forward's log-sum-exp and dS = alpha P o (drop(dP) - D):
+//   MODE 0 (CTA = 128 queries): D = rowsum(dO o O);  per 64-key block: S = Q K^T, dP = dO V^T -> dS -> dQ += dS K
+//   MODE 1 (CTA = 128 keys)   : per 64-query block: S^T = K Q^T, dP^T = V dO^T -> Pdrop^T, dS^T
+//                               -> dV += Pdrop^T dO, dK += dS^T Q
+// MODE 1 forms the transposed products directly, so its fragments have keys as rows and feed the accumulating
+// products as register A operands without any transposition.  No atomics.
 struct BwdParams {
   const bf16 *o, *dout;
   bf16 *dq, *dk, *dv;
@@ -698,354 +275,238 @@ struct BwdParams {
   float scale;
 };
 
+// tr0 / tr1: the CTA's resident 128-row tiles (Q, dO for MODE 0; K, V for MODE 1), box 128 rows;
+// ts0 / ts1: the streamed 64-row blocks (K, V for MODE 0; Q, dO for MODE 1), box 64 rows.
 template <int MODE>
 __global__ void __launch_bounds__(NT, 1)
-attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
-                   const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
+attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constant__ CUtensorMap tr1,
+                   const __grid_constant__ CUtensorMap ts0, const __grid_constant__ CUtensorMap ts1, const BwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sR0 = smem;                          // resident: Q_i (MODE 0) / K_t (MODE 1)
-  uint8_t* sR1 = sR0 + TILE_BYTES;              // resident: dO_i       / V_t
-  uint8_t* sST = sR1 + TILE_BYTES;              // 2 stages x (K_j | V_j) or (Q_i | dO_i)
-  uint8_t* sPD = sST + 4 * TILE_BYTES;          // Pdrop tile: 2 key blocks x [128 q][64 k]   (MODE 1)
-  uint8_t* sDS = sPD + 2 * TILE_BYTES;          // dS tile, same layout
-  float* skm = reinterpret_cast<float*>(sDS + 2 * TILE_BYTES);   // [2][128] log2-domain key mask per stage / tile
-  float* srow = skm + 256;                                         // [128] dsum exchange (MODE 0)
-  float* skf = srow + 128;                                         // [2][4] per 32-key chunk: mask not identically zero
-  uint64_t* bars = reinterpret_cast<uint64_t*>(skf + 8);
-  uint64_t* r_full = bars + 0;
-  uint64_t* st_full = bars + 1;     // [2]
-  uint64_t* st_empty = bars + 3;    // [2]
-  uint64_t* sdp_full = bars + 5;
-  uint64_t* sdp_empty = bars + 6;
-  uint64_t* ds_full = bars + 7;
-  uint64_t* ds_empty = bars + 8;
-  uint64_t* acc_full = bars + 9;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 10);
+  uint8_t* sR0 = smem;
+  uint8_t* sR1 = sR0 + R_BYTES;
+  uint8_t* sS0 = sR1 + R_BYTES;             // [NST] streamed block 0 (K_j / Q_i)
+  uint8_t* sS1 = sS0 + NST * BLK_BYTES;     // [NST] streamed block 1 (V_j / dO_i)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sS1 + NST * BLK_BYTES);
+  uint64_t* r_full = bars;
+  uint64_t* st_full = bars + 1;          // [NST]
+  uint64_t* st_free = bars + 1 + NST;    // [NST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t0 = blockIdx.x * BM, h = blockIdx.y, b = blockIdx.z;   // first query (MODE 0) / key (MODE 1) of this CTA
-  const int ntiles = MODE == 0 ? (p.nk + BM - 1) / BM : (p.nq + BM - 1) / BM;
+  const int nblk = MODE == 0 ? (p.nk + KB - 1) / KB : (p.nq + KB - 1) / KB;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tq);
-      tma_prefetch_desc(&tk);
-      tma_prefetch_desc(&tv);
-      tma_prefetch_desc(&tdo);
-      mbar_init(r_full, 1);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&st_full[i], 1);
-        mbar_init(&st_empty[i], 1);
-      }
-      mbar_init(sdp_full, 1);
-      mbar_init(sdp_empty, 256);
-      mbar_init(ds_full, 256);
-      mbar_init(ds_empty, 1);
-      mbar_init(acc_full, 1);
-      fence_mbar_init();
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tr0);
+    tma_prefetch_desc(&tr1);
+    tma_prefetch_desc(&ts0);
+    tma_prefetch_desc(&ts1);
+    mbar_init(r_full, 1);
+    for (int i = 0; i < NST; ++i) {
+      mbar_init(&st_full[i], 1);
+      mbar_init(&st_free[i], 8);
     }
-    __syncwarp();
-    tmem_alloc(tmem_ptr_smem, 512);
-    tmem_relinquish();
+    fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
-      // resident operands
-      mbar_expect_tx(r_full, 2 * TILE_BYTES);
-      if (MODE == 0) {
-        tma_load_4d(sR0, &tq, r_full, 0, t0, h, b);
-        tma_load_4d(sR1, &tdo, r_full, 0, t0, h, b);
-      } else {
-        tma_load_4d(sR0, &tk, r_full, 0, t0, h, b);
-        tma_load_4d(sR1, &tv, r_full, 0, t0, h, b);
+      mbar_expect_tx(r_full, 2 * R_BYTES);
+      tma_load_4d(sR0, &tr0, r_full, 0, t0, h, b);
+      tma_load_4d(sR1, &tr1, r_full, 0, t0, h, b);
+      for (int j = 0; j < nblk; ++j) {
+        const int st = j % NST;
+        mbar_wait_relaxed(&st_free[st], ((j / NST) & 1) ^ 1);
+        mbar_expect_tx(&st_full[st], 2 * BLK_BYTES);
+        tma_load_4d(sS0 + st * BLK_BYTES, &ts0, &st_full[st], 0, j * KB, h, b);
+        tma_load_4d(sS1 + st * BLK_BYTES, &ts1, &st_full[st], 0, j * KB, h, b);
       }
-      auto load_stage = [&](int tile) {
-        const int s = tile & 1;
-        uint8_t* d0 = sST + s * 2 * TILE_BYTES;
-        mbar_expect_tx(&st_full[s], 2 * TILE_BYTES);
-        if (MODE == 0) {
-          tma_load_4d(d0, &tk, &st_full[s], 0, tile * BM, h, b);
-          tma_load_4d(d0 + TILE_BYTES, &tv, &st_full[s], 0, tile * BM, h, b);
-        } else {
-          tma_load_4d(d0, &tq, &st_full[s], 0, tile * BM, h, b);
-          tma_load_4d(d0 + TILE_BYTES, &tdo, &st_full[s], 0, tile * BM, h, b);
-        }
-      };
-      load_stage(0);
-      const uint32_t idesc_s = umma_idesc_bf16(BM, 128, 0, 0);
-      const uint32_t idesc_acc = MODE == 0 ? umma_idesc_bf16(BM, 64, 0, 1) : umma_idesc_bf16(BM, 64, 1, 1);
-      const uint32_t aR0 = smem_u32(sR0), aR1 = smem_u32(sR1), aPD = smem_u32(sPD), aDS = smem_u32(sDS);
-      mbar_wait_relaxed(r_full, 0);
-      // accumulate the products of tile t (its Pdrop / dS are in shared memory, its streamed operands in stage t & 1)
-      auto issue_acc = [&](int t) {
-        const uint32_t a0 = smem_u32(sST + (t & 1) * 2 * TILE_BYTES), a1 = a0 + TILE_BYTES;
-        mbar_wait_relaxed(ds_full, t & 1);
-        tc_fence_after();
-        if (MODE == 0) {
-          // dQ += dS K_j : A = dS K-major (two 64-key blocks), B = K_j [key][d] as MN-major (N = d, K = key)
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_bf16_ss(tmem_base + B_ACC0, umma_smem_desc(aDS + (kk >> 2) * TILE_BYTES + (kk & 3) * 32, 16, 1024),
-                         umma_smem_desc(a0 + kk * 2048, 8192, 1024), idesc_acc, (t > 0 || kk > 0) ? 1u : 0u);
-        } else {
-          // dV += Pdrop^T dO_i, dK += dS^T Q_i : A = [q][key] tile read MN-major (M = key, K = q), B = [q][d] MN-major
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_bf16_ss(tmem_base + B_ACC0, umma_smem_desc(aPD + kk * 2048, TILE_BYTES, 1024),
-                         umma_smem_desc(a1 + kk * 2048, 8192, 1024), idesc_acc, (t > 0 || kk > 0) ? 1u : 0u);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_bf16_ss(tmem_base + B_ACC1, umma_smem_desc(aDS + kk * 2048, TILE_BYTES, 1024),
-                         umma_smem_desc(a0 + kk * 2048, 8192, 1024), idesc_acc, (t > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(ds_empty);
-        umma_commit(&st_empty[t & 1]);
-      };
-      for (int tile = 0; tile < ntiles; ++tile) {
-        const int s = tile & 1;
-        mbar_wait_relaxed(&st_full[s], (tile >> 1) & 1);
-        if (tile > 0) mbar_wait_relaxed(sdp_empty, (tile - 1) & 1);   // the softmax warps hold S / dP of tile-1 in registers
-        tc_fence_after();
-        const uint32_t a0 = smem_u32(sST + s * 2 * TILE_BYTES), a1 = a0 + TILE_BYTES;
-        // S = Q K^T and dP = dO V^T (both operands K-major, N = 128)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t dq_ = umma_smem_desc((MODE == 0 ? aR0 : a0) + k * 32, 16, 1024);
-          const uint64_t dk_ = umma_smem_desc((MODE == 0 ? a0 : aR0) + k * 32, 16, 1024);
-          umma_bf16_ss(tmem_base + B_S_COL, dq_, dk_, idesc_s, k > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t ddo = umma_smem_desc((MODE == 0 ? aR1 : a1) + k * 32, 16, 1024);
-          const uint64_t dv_ = umma_smem_desc((MODE == 0 ? a1 : aR1) + k * 32, 16, 1024);
-          umma_bf16_ss(tmem_base + B_DP_COL, ddo, dv_, idesc_s, k > 0 ? 1u : 0u);
-        }
-        umma_commit(sdp_full);
-        // while the softmax warps work on this tile: finish the previous one and fetch the next
-        if (tile > 0) issue_acc(tile - 1);
-        if (tile + 1 < ntiles) {
-          if (tile >= 1) mbar_wait_relaxed(&st_empty[s ^ 1], ((tile - 1) >> 1) & 1);
-          load_stage(tile + 1);
-        }
-      }
-      issue_acc(ntiles - 1);
-      umma_commit(acc_full);
     }
-    __syncwarp();
+    return;
+  }
+
+  const int wg = warp >> 2;
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t t16s = p.thresh & 0xFFFF0000u;
+  const float scale_eff = p.thresh ? p.scale : 1.0f, inv_scale = 1.0f / scale_eff, as_ = p.alpha * scale_eff;
+  const int64_t bh = (int64_t)b * p.H + h;
+  const uint32_t aR0 = smem_u32(sR0) + wg * 8192, aR1 = smem_u32(sR1) + wg * 8192;
+  int row[2];   // this thread's two rows: queries (MODE 0) / keys (MODE 1)
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) row[hh] = t0 + wg * 64 + r0 + 8 * hh;
+
+  // per-row state: MODE 0 -> -lse, D / scale and the dropout row hash of the query; MODE 1 -> key mask of the key
+  float rs_a[2], rs_b[2];
+  uint32_t rh[2] = {0u, 0u};
+  if (MODE == 0) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int qq = row[hh];
+      const bool ok = qq < p.nq;
+      // D = rowsum(dO o O): each thread of the quad covers 16 of the 64 columns
+      float acc = 0.f;
+      if (ok) {
+        const uint4* po = reinterpret_cast<const uint4*>(p.o + (int64_t)b * p.o_bs + (int64_t)qq * p.ldo + h * 64 + (lane & 3) * 16);
+        const uint4* pd = reinterpret_cast<const uint4*>(p.dout + (int64_t)b * p.do_bs + (int64_t)qq * p.lddo + h * 64 + (lane & 3) * 16);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const uint4 a = __ldg(po + i), d = __ldg(pd + i);
+          const __nv_bfloat162* ap = reinterpret_cast<const __nv_bfloat162*>(&a);
+          const __nv_bfloat162* dp = reinterpret_cast<const __nv_bfloat162*>(&d);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float2 x = __bfloat1622float2(ap[e]), y = __bfloat1622float2(dp[e]);
+            acc = fmaf(x.x, y.x, acc);
+            acc = fmaf(x.y, y.y, acc);
+          }
+        }
+      }
+      acc = quad_sum(acc);
+      if (ok && (lane & 3) == 0) p.dsum[bh * p.nq + qq] = acc;
+      rs_a[hh] = ok ? -__ldg(p.lse + bh * p.nq + qq) : -INFINITY;
+      rs_b[hh] = acc * inv_scale;
+      rh[hh] = p.thresh ? rng_u32(p.seed, (uint64_t)(bh * p.nq + qq)) : 0u;
+    }
   } else {
-    const int quarter = warp & 3;
-    const int hf = (warp - 1) >> 2;           // key columns [64 hf, 64 hf + 64) of every tile
-    const int row = quarter * 32 + lane;      // query row of the tile = TMEM lane
-    const int st = threadIdx.x - 32;
-    const uint32_t trow = tmem_base + (uint32_t(quarter * 32) << 16);
-    const uint32_t t16s = p.thresh & 0xFFFF0000u;
-    const float scale_eff = p.thresh ? p.scale : 1.0f, inv_scale = 1.0f / scale_eff, as_ = p.alpha * scale_eff;
-    const int sw = row & 7;
-    const uint32_t rowoff = hf * TILE_BYTES + (row >> 3) * 1024 + (row & 7) * 128;
-    const uint32_t a_skm = smem_u32(skm), a_srow = smem_u32(srow), a_sDS = smem_u32(sDS), a_sPD = smem_u32(sPD);
-    const uint32_t a_skf = smem_u32(skf);
-    // per-row state of the CURRENT query tile
-    float lse_r = INFINITY, dsum_r = 0.f;
-    uint32_t rh = 0;
-    auto load_row_state = [&](int q) {        // q = global query index of this thread's row
-      const int64_t gr = ((int64_t)b * p.H + h) * p.nq + q;
-      if (q < p.nq) {
-        lse_r = __ldg(p.lse + gr);
-        if (MODE == 1) dsum_r = __ldg(p.dsum + gr);
-      } else {
-        lse_r = INFINITY;
-        dsum_r = 0.f;
-      }
-      rh = p.thresh ? rng_u32(p.seed, (uint64_t)gr) : 0u;
-    };
-    if (MODE == 0) {
-      load_row_state(t0 + row);
-      // D = rowsum(dO o O) for this row, shared with the other key half through smem and saved for MODE 1
-      if (hf == 0) {
-        float acc = 0.f;
-        if (t0 + row < p.nq) {
-          const uint4* po = reinterpret_cast<const uint4*>(p.o + (int64_t)b * p.o_bs + (int64_t)(t0 + row) * p.ldo + h * 64);
-          const uint4* pd = reinterpret_cast<const uint4*>(p.dout + (int64_t)b * p.do_bs + (int64_t)(t0 + row) * p.lddo + h * 64);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const uint4 a = __ldg(po + i), d = __ldg(pd + i);
-            const __nv_bfloat162* ap = reinterpret_cast<const __nv_bfloat162*>(&a);
-            const __nv_bfloat162* dp = reinterpret_cast<const __nv_bfloat162*>(&d);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 x = __bfloat1622float2(ap[e]), y = __bfloat1622float2(dp[e]);
-              acc = fmaf(x.x, y.x, acc);
-              acc = fmaf(x.y, y.y, acc);
-            }
-          }
-          p.dsum[((int64_t)b * p.H + h) * p.nq + t0 + row] = acc;
-        }
-        sts_f(a_srow + row * 4, acc);
-      }
-      named_sync_256();
-      dsum_r = lds_f(a_srow + row * 4);
-    }
-
-    for (int tile = 0; tile < ntiles; ++tile) {
-      const int key0 = MODE == 0 ? tile * BM : t0;
-      uint32_t km = a_skm + (tile & 1) * 512;
-      if (MODE == 1) load_row_state(tile * BM + row);
-      if (MODE == 0 || tile == 0) {
-        if (st < 128) {
-          const int col = key0 + st;
-          const float kv = col < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + col) * LOG2E : 0.f) : -INFINITY;
-          sts_f(km + st * 4, kv);
-          const bool any = __any_sync(0xffffffffu, kv != 0.f);
-          if (lane == 0) sts_f(a_skf + ((tile & 1) * 4 + (st >> 5)) * 4, any ? 1.f : 0.f);
-        }
-        named_sync_256();
-      } else {
-        km = a_skm;
-      }
-      mbar_wait(sdp_full, tile & 1);
-      tc_fence_after();
-      // this thread's 64 score and 64 dP columns -> registers, then TMEM is released: the next tile's S / dP products
-      // run on the tensor pipe while this tile's element-wise work proceeds
-      uint32_t rs[64], rp[64];
-      {
-        uint32_t(&s0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&rs[0]);
-        uint32_t(&s1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&rs[32]);
-        uint32_t(&p0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&rp[0]);
-        uint32_t(&p1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&rp[32]);
-        tmem_ld32(trow + B_S_COL + hf * 64, s0);
-        tmem_ld32(trow + B_S_COL + hf * 64 + 32, s1);
-        tmem_ld32(trow + B_DP_COL + hf * 64, p0);
-        tmem_ld32(trow + B_DP_COL + hf * 64 + 32, p1);
-        tmem_ld_wait32(s0);
-        tmem_ld_wait32(s1);
-        tmem_ld_wait32(p0);
-        tmem_ld_wait32(p1);
-      }
-      tc_fence_before();
-      mbar_arrive(sdp_empty);
-      if (tile > 0) mbar_wait(ds_empty, (tile - 1) & 1);      // the previous tile's Pdrop / dS have been consumed
-      const float nlse = -lse_r;
-      const float dsum_s = dsum_r * inv_scale;                // dS = (alpha scale) P o (keep ? dP : 0  -  D / scale)
-#pragma unroll
-      for (int c = 0; c < 64; c += 32) {
-        const int col0 = hf * 64 + c;
-        const bool masked = lds_f(a_skf + ((MODE == 0 ? (tile & 1) : 0) * 4 + (col0 >> 5)) * 4) != 0.f;
-        const uint32_t km4 = km + col0 * 4;
-        const uint32_t pair0 = (uint32_t)(key0 + col0) >> 1;
-#pragma unroll
-        for (int i = 0; i < 8; i += 2) {
-          uint32_t ws[4], wp[4];
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int e0 = c + 4 * (i + u);
-            float pe[4];
-            if (masked) {
-              const float4 kmv = lds_f4(km4 + (i + u) * 16);
-              pe[0] = ex2f(fmaf(__uint_as_float(rs[e0 + 0]), p.a2, kmv.x + nlse));
-              pe[1] = ex2f(fmaf(__uint_as_float(rs[e0 + 1]), p.a2, kmv.y + nlse));
-              pe[2] = ex2f(fmaf(__uint_as_float(rs[e0 + 2]), p.a2, kmv.z + nlse));
-              pe[3] = ex2f(fmaf(__uint_as_float(rs[e0 + 3]), p.a2, kmv.w + nlse));
-            } else {
-              pe[0] = ex2f(fmaf(__uint_as_float(rs[e0 + 0]), p.a2, nlse));
-              pe[1] = ex2f(fmaf(__uint_as_float(rs[e0 + 1]), p.a2, nlse));
-              pe[2] = ex2f(fmaf(__uint_as_float(rs[e0 + 2]), p.a2, nlse));
-              pe[3] = ex2f(fmaf(__uint_as_float(rs[e0 + 3]), p.a2, nlse));
-            }
-            float ge[4] = {__uint_as_float(rp[e0 + 0]), __uint_as_float(rp[e0 + 1]), __uint_as_float(rp[e0 + 2]),
-                           __uint_as_float(rp[e0 + 3])};
-            float pd[4] = {pe[0], pe[1], pe[2], pe[3]};
-            if (p.thresh) {
-              const uint32_t x0 = mix_pair(rh, pair0 + 2 * (i + u)), x1 = mix_pair(rh, pair0 + 2 * (i + u) + 1);
-              const bool k0 = (x0 << 16) >= t16s, k1 = x0 >= t16s, k2 = (x1 << 16) >= t16s, k3 = x1 >= t16s;
-              ge[0] = k0 ? ge[0] : 0.f;
-              ge[1] = k1 ? ge[1] : 0.f;
-              ge[2] = k2 ? ge[2] : 0.f;
-              ge[3] = k3 ? ge[3] : 0.f;
-              if (MODE == 1) {
-                pd[0] = k0 ? pe[0] : 0.f;
-                pd[1] = k1 ? pe[1] : 0.f;
-                pd[2] = k2 ? pe[2] : 0.f;
-                pd[3] = k3 ? pe[3] : 0.f;
-              }
-            }
-            ws[2 * u] = pack2((pe[0] * as_) * (ge[0] - dsum_s), (pe[1] * as_) * (ge[1] - dsum_s));
-            ws[2 * u + 1] = pack2((pe[2] * as_) * (ge[2] - dsum_s), (pe[3] * as_) * (ge[3] - dsum_s));
-            if (MODE == 1) {
-              wp[2 * u] = pack2(pd[0], pd[1]);
-              wp[2 * u + 1] = pack2(pd[2], pd[3]);
-            }
-          }
-          const uint32_t off = rowoff + ((((c >> 3) + (i >> 1)) ^ sw) << 4);
-          sts_u4(a_sDS + off, ws[0], ws[1], ws[2], ws[3]);
-          if (MODE == 1) sts_u4(a_sPD + off, wp[0], wp[1], wp[2], wp[3]);
-        }
-      }
-      fence_proxy_async();
-      mbar_arrive(ds_full);
-    }
-
-    // ---- accumulators -> bf16 rows (MODE 0: dQ rows = queries; MODE 1: dV / dK rows = keys)
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    const int nrows = MODE == 0 ? p.nq : p.nk;
-    const bool valid = t0 + row < nrows;
-    auto store32 = [&](uint32_t col, bf16* dst, float mul) {   // the TMEM load is warp-collective: only the store is predicated
-      uint32_t r[32];
-      tmem_ld32(trow + col, r);
-      tmem_ld_wait32(r);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * mul);
-      if (valid) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          reinterpret_cast<uint4*>(dst)[i] =
-              make_uint4(pack2(__uint_as_float(r[8 * i]), __uint_as_float(r[8 * i + 1])),
-                         pack2(__uint_as_float(r[8 * i + 2]), __uint_as_float(r[8 * i + 3])),
-                         pack2(__uint_as_float(r[8 * i + 4]), __uint_as_float(r[8 * i + 5])),
-                         pack2(__uint_as_float(r[8 * i + 6]), __uint_as_float(r[8 * i + 7])));
-      }
-    };
-    const int64_t grow_ = t0 + row;
-    if (MODE == 0) {
-      store32(B_ACC0 + hf * 32, p.dq + (int64_t)b * p.dq_bs + grow_ * p.lddq + h * 64 + hf * 32, 1.0f);
-    } else {
-      store32(B_ACC0 + hf * 32, p.dv + (int64_t)b * p.dv_bs + grow_ * p.lddv + h * 64 + hf * 32, scale_eff);   // Pdrop unscaled
-      store32(B_ACC1 + hf * 32, p.dk + (int64_t)b * p.dk_bs + grow_ * p.lddk + h * 64 + hf * 32, 1.0f);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int kk = row[hh];
+      rs_a[hh] = kk < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + kk) * LOG2E : 0.f) : -INFINITY;
+      rs_b[hh] = 0.f;
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  float acc0[32], acc1[32];   // dQ (MODE 0) / dV, dK (MODE 1)
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc0[i] = acc1[i] = 0.f;
+  mbar_wait(r_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % NST;
+    mbar_wait(&st_full[st], (j / NST) & 1);
+    const uint32_t a0 = smem_u32(sS0 + st * BLK_BYTES), a1 = smem_u32(sS1 + st * BLK_BYTES);
+    float s[32], g[32];
+    fence_regs(s);
+    fence_regs(g);
+    wgmma_fence();
+    qk_product(s, aR0, a0);   // S = Q K^T (MODE 0) / S^T = K Q^T (MODE 1)
+    qk_product(g, aR1, a1);   // dP = dO V^T        / dP^T = V dO^T
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    fence_regs(g);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int c = j * KB + 8 * jj + cq;
+      // per-column state: MODE 0 -> key mask; MODE 1 -> -lse, D / scale and the dropout hash of the query
+      float ca[2], cb[2] = {0.f, 0.f};
+      uint32_t ch[2] = {0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        if (MODE == 0) {
+          ca[e] = c + e < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + c + e) * LOG2E : 0.f) : -INFINITY;
+        } else {
+          const bool ok = c + e < p.nq;
+          ca[e] = ok ? -__ldg(p.lse + bh * p.nq + c + e) : -INFINITY;
+          cb[e] = ok ? __ldg(p.dsum + bh * p.nq + c + e) * inv_scale : 0.f;
+          ch[e] = p.thresh ? rng_u32(p.seed, (uint64_t)(bh * p.nq + c + e)) : 0u;
+        }
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float pe[2], pd[2], ds[2];
+        // the dropout hash is keyed by (query, key pair): MODE 0 rows are queries, MODE 1 rows are keys
+        const uint32_t x = p.thresh ? (MODE == 0 ? mix_pair(rh[hh], (uint32_t)c >> 1) : 0u) : 0u;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int i = 4 * jj + 2 * hh + e;
+          float gv = g[i];
+          float dsub;
+          if (MODE == 0) {
+            pe[e] = ex2f(fmaf(s[i], p.a2, ca[e] + rs_a[hh]));
+            dsub = rs_b[hh];
+            pd[e] = pe[e];
+            if (p.thresh && !keep_key(x, c + e, t16s)) gv = 0.f;
+          } else {
+            pe[e] = ex2f(fmaf(s[i], p.a2, rs_a[hh] + ca[e]));
+            dsub = cb[e];
+            pd[e] = pe[e];
+            if (p.thresh) {
+              const uint32_t xk = mix_pair(ch[e], (uint32_t)row[hh] >> 1);
+              if (!keep_key(xk, row[hh], t16s)) {
+                gv = 0.f;
+                pd[e] = 0.f;
+              }
+            }
+          }
+          ds[e] = (pe[e] * as_) * (gv - dsub);
+        }
+        s[4 * jj + 2 * hh] = pd[0];
+        s[4 * jj + 2 * hh + 1] = pd[1];
+        g[4 * jj + 2 * hh] = ds[0];
+        g[4 * jj + 2 * hh + 1] = ds[1];
+      }
+    }
+    uint32_t fds[4][4];
+    to_afrag(g, fds);
+    fence_regs(acc0);
+    fence_regs(acc1);
+    wgmma_fence();
+    if (MODE == 0) {
+      pv_product(acc0, fds, a0);            // dQ += dS K_j
+    } else {
+      uint32_t fpd[4][4];
+      to_afrag(s, fpd);
+      pv_product(acc0, fpd, a1);            // dV += Pdrop^T dO_i
+      pv_product(acc1, fds, a0);            // dK += dS^T Q_i
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc0);
+    fence_regs(acc1);
+    if (lane == 0) mbar_arrive(&st_free[st]);
+  }
+
+  // ---- accumulators -> bf16 rows (MODE 0: dQ rows = queries; MODE 1: dV / dK rows = keys)
+  const int nrows = MODE == 0 ? p.nq : p.nk;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int64_t r = row[hh];
+    if (r >= nrows) continue;
+    if (MODE == 0) {
+      bf16* dst = p.dq + (int64_t)b * p.dq_bs + r * p.lddq + h * 64 + cq;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) store_row_pair(dst + 8 * jj, acc0[4 * jj + 2 * hh], acc0[4 * jj + 2 * hh + 1]);
+    } else {
+      bf16* dv = p.dv + (int64_t)b * p.dv_bs + r * p.lddv + h * 64 + cq;   // Pdrop is unscaled
+      bf16* dk = p.dk + (int64_t)b * p.dk_bs + r * p.lddk + h * 64 + cq;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        store_row_pair(dv + 8 * jj, acc0[4 * jj + 2 * hh] * scale_eff, acc0[4 * jj + 2 * hh + 1] * scale_eff);
+        store_row_pair(dk + 8 * jj, acc1[4 * jj + 2 * hh], acc1[4 * jj + 2 * hh + 1]);
+      }
+    }
   }
 }
 
-static int g_smem_optin = 0;
+constexpr size_t FWD_SMEM = 1024 + R_BYTES + 2 * (size_t)NST * BLK_BYTES + (1 + 2 * NST) * 8;
+constexpr size_t BWD_SMEM = 1024 + 2 * R_BYTES + 2 * (size_t)NST * BLK_BYTES + (1 + 2 * NST) * 8;
+
+static int g_init = 0;
 static int init_once() {
-  if (g_smem_optin) return 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return set_error("cudaGetDevice failed");
-  cudaDeviceGetAttribute(&g_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  if (cudaFuncSetAttribute(attn_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) != cudaSuccess ||
-      cudaFuncSetAttribute(attn_tc_fwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) != cudaSuccess ||
-      cudaFuncSetAttribute(attn_tc_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) != cudaSuccess ||
-      cudaFuncSetAttribute(attn_tc_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) != cudaSuccess)
+  if (g_init) return 0;
+  if (cudaFuncSetAttribute(attn_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(attn_tc_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(attn_tc_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM) != cudaSuccess)
     return set_error("cudaFuncSetAttribute failed for the attn_tc kernels");
+  g_init = 1;
   return 0;
 }
 
 // BB_ATTN_TC: 0 = never, 1 (default) = when nk >= 64, 2 = whenever the kernel supports the call (tests)
-static long long* g_trace = nullptr;
 static int g_tc_mode = -1;
 int tc_mode() {
   if (g_tc_mode < 0) {
@@ -1072,55 +533,20 @@ bool fwd_supported(const bb_flash_args* a) {
   return true;
 }
 
-static int fwd_version() {      // BB_ATTN_FWD=1 selects the first-generation kernel (whole key range in TMEM)
-  static const int v = [] {
-    const char* e = getenv("BB_ATTN_FWD");
-    return e ? atoi(e) : 2;
-  }();
-  return v;
-}
-
 int launch_fwd(const bb_flash_args* a, void* stream) {
   if (int e = init_once()) return e;
   FwdParams p;
   memset(&p, 0, sizeof(p));
-  if (fwd_version() == 2 && a->nk <= 4096) {
-    p.out = (bf16*)a->o; p.o_bs = a->o_bs; p.ldo = a->ldo; p.lse = a->lse; p.kmask = a->kmask;
-    p.B = a->B; p.H = a->H; p.nq = a->nq; p.nk = a->nk;
-    p.a2 = a->alpha * LOG2E;
-    p.seed = a->seed; p.thresh = a->thresh; p.scale = a->scale;
-    p.trace = nullptr;
-    CUtensorMap tq, tk, tv;
-    if (int e = make_tmap_bf16_4d(&tq, a->q, 64, a->nq, a->H, a->B, a->ldq, 64, a->q_bs, BM)) return e;
-    if (int e = make_tmap_bf16_4d(&tk, a->k, 64, a->nk, a->H, a->B, a->ldk, 64, a->k_bs, KB)) return e;
-    if (int e = make_tmap_bf16_4d(&tv, a->v, 64, a->nk, a->H, a->B, a->ldv, 64, a->v_bs, KB)) return e;
-    const int nblk = (a->nk + KB - 1) / KB;
-    const size_t smem = 1024 + Q_BYTES + 2 * (size_t)F2_KST * BLK_BYTES + 2 * P_BYTES + (size_t)nblk * KB * 4 +
-                        (size_t)((nblk * 2 + 3) & ~3) * 4 + 2 * BM * 4 + 24 * 8 + 64;
-    const dim3 grid((unsigned)((a->nq + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
-    launch_pdl(attn_tc_fwd2_kernel, grid, dim3(F2_NT), smem, (cudaStream_t)stream, tq, tk, tv, p);
-    count_launch();
-    return check_launch("attn_tc_fwd2_kernel");
-  }
   p.out = (bf16*)a->o; p.o_bs = a->o_bs; p.ldo = a->ldo; p.lse = a->lse; p.kmask = a->kmask;
   p.B = a->B; p.H = a->H; p.nq = a->nq; p.nk = a->nk;
-  p.nsb = (a->nk + MAX_SBK - 1) / MAX_SBK;
-  p.sbk = (((a->nk + p.nsb - 1) / p.nsb) + KB - 1) / KB * KB;
-  p.nsb = (a->nk + p.sbk - 1) / p.sbk;
   p.a2 = a->alpha * LOG2E;
   p.seed = a->seed; p.thresh = a->thresh; p.scale = a->scale;
-  const int need = S_COL + p.sbk;
-  p.tmem_cols = need <= 128 ? 128 : (need <= 256 ? 256 : 512);
-  p.trace = g_trace;
   CUtensorMap tq, tk, tv;
   if (int e = make_tmap_bf16_4d(&tq, a->q, 64, a->nq, a->H, a->B, a->ldq, 64, a->q_bs, BM)) return e;
   if (int e = make_tmap_bf16_4d(&tk, a->k, 64, a->nk, a->H, a->B, a->ldk, 64, a->k_bs, KB)) return e;
   if (int e = make_tmap_bf16_4d(&tv, a->v, 64, a->nk, a->H, a->B, a->ldv, 64, a->v_bs, KB)) return e;
-  const int nkb = p.sbk / KB;
-  const size_t smem = 1024 + Q_BYTES + 2 * (size_t)nkb * BLK_BYTES + 2 * P_BYTES + (size_t)p.sbk * 4 + 4 * BM * 4 + 64 + 128;
-  if ((int)smem > g_smem_optin) return set_error("attn_tc_fwd: shared memory budget exceeded");
   const dim3 grid((unsigned)((a->nq + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
-  launch_pdl(attn_tc_fwd_kernel, grid, dim3(NT), smem, (cudaStream_t)stream, tq, tk, tv, p);
+  launch_pdl(attn_tc_fwd_kernel, grid, dim3(NT), FWD_SMEM, (cudaStream_t)stream, tq, tk, tv, p);
   count_launch();
   return check_launch("attn_tc_fwd_kernel");
 }
@@ -1147,17 +573,19 @@ int launch_bwd(const bb_flash_args* a, void* stream) {
   p.B = a->B; p.H = a->H; p.nq = a->nq; p.nk = a->nk;
   p.a2 = a->alpha * LOG2E; p.alpha = a->alpha;
   p.seed = a->seed; p.thresh = a->thresh; p.scale = a->scale;
-  CUtensorMap tq, tk, tv, tdo;
+  CUtensorMap tq, tk, tv, tdo, tq64, tk64, tv64, tdo64;
   if (int e = make_tmap_bf16_4d(&tq, a->q, 64, a->nq, a->H, a->B, a->ldq, 64, a->q_bs, BM)) return e;
+  if (int e = make_tmap_bf16_4d(&tdo, a->dout, 64, a->nq, a->H, a->B, a->lddo, 64, a->do_bs, BM)) return e;
   if (int e = make_tmap_bf16_4d(&tk, a->k, 64, a->nk, a->H, a->B, a->ldk, 64, a->k_bs, BM)) return e;
   if (int e = make_tmap_bf16_4d(&tv, a->v, 64, a->nk, a->H, a->B, a->ldv, 64, a->v_bs, BM)) return e;
-  if (int e = make_tmap_bf16_4d(&tdo, a->dout, 64, a->nq, a->H, a->B, a->lddo, 64, a->do_bs, BM)) return e;
-  const size_t smem = 1024 + 10 * (size_t)TILE_BYTES + 392 * 4 + 128;
-  if ((int)smem > g_smem_optin) return set_error("attn_tc_bwd: shared memory budget exceeded");
+  if (int e = make_tmap_bf16_4d(&tq64, a->q, 64, a->nq, a->H, a->B, a->ldq, 64, a->q_bs, KB)) return e;
+  if (int e = make_tmap_bf16_4d(&tdo64, a->dout, 64, a->nq, a->H, a->B, a->lddo, 64, a->do_bs, KB)) return e;
+  if (int e = make_tmap_bf16_4d(&tk64, a->k, 64, a->nk, a->H, a->B, a->ldk, 64, a->k_bs, KB)) return e;
+  if (int e = make_tmap_bf16_4d(&tv64, a->v, 64, a->nk, a->H, a->B, a->ldv, 64, a->v_bs, KB)) return e;
   const dim3 gq((unsigned)((a->nq + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
   const dim3 gk((unsigned)((a->nk + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
-  launch_pdl(attn_tc_bwd_kernel<0>, gq, dim3(NT), smem, (cudaStream_t)stream, tq, tk, tv, tdo, p);
-  launch_pdl(attn_tc_bwd_kernel<1>, gk, dim3(NT), smem, (cudaStream_t)stream, tq, tk, tv, tdo, p);
+  launch_pdl(attn_tc_bwd_kernel<0>, gq, dim3(NT), BWD_SMEM, (cudaStream_t)stream, tq, tdo, tk64, tv64, p);
+  launch_pdl(attn_tc_bwd_kernel<1>, gk, dim3(NT), BWD_SMEM, (cudaStream_t)stream, tk, tv, tq64, tdo64, p);
   count_launch(2);
   return check_launch("attn_tc_bwd kernels");
 }
@@ -1166,8 +594,9 @@ int launch_bwd(const bb_flash_args* a, void* stream) {
 }  // namespace bb
 
 extern "C" int bb_set_attn_tc(int mode) { return bb::fat::set_tc_mode(mode); }
+// kept for the C ABI: the wgmma kernels record no per-CTA trace
 extern "C" int bb_attn_tc_trace(long long* device_buf) {
-  bb::fat::g_trace = device_buf;
+  (void)device_buf;
   return 0;
 }
 

@@ -1,4 +1,4 @@
-// tcgen05 / TMA attention core (attn_tc.cu), dispatched from bb_flash_fwd / bb_flash_bwd (attn_flash.cu).
+// wgmma / TMA attention core (attn_tc.cu), dispatched from bb_flash_fwd / bb_flash_bwd (attn_flash.cu).
 #pragma once
 #include "../../include/bevbert_b200.h"
 

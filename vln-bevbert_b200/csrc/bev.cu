@@ -1,4 +1,4 @@
-// BEV grid lifting for sm_100a: depth un-projection + camera->world->ego transforms + integer cell index
+// BEV grid lifting for sm_90a: depth un-projection + camera->world->ego transforms + integer cell index
 // (one pass, bit-exact arithmetic order), then a deterministic scatter-mean pool of 768-wide patch
 // features (and float64 semantic one-hots) into the D x D metric map.
 //

@@ -1,6 +1,6 @@
 // High-precision verification arm of the GEMM entry point: when the library is in fp32-activation mode
 // (bb_set_act_f32(1)), bb_gemm_bf16 dispatches here.  Same argument struct, same operand-major / batch-stride /
-// epilogue semantics as the tcgen05 kernel (gemm_tc.cu), but A, B, aux, add_in and D are fp32 and every product is an
+// epilogue semantics as the wgmma kernel (gemm_tc.cu), but A, B, aux, add_in and D are fp32 and every product is an
 // fp32 FMA on the CUDA cores.  It exists to separate kernel LOGIC from bf16 PRECISION in the parity tests (north_star
 // "1e-3 rel fp32"): throughput is irrelevant here (a plain 64 x 64 shared-memory tiling), results are deterministic.
 #include <cuda_runtime.h>

@@ -1,11 +1,13 @@
-// Batched bf16 GEMM for sm_100a: TMA -> 128B-swizzled shared memory -> tcgen05.mma (fp32 accumulators
-// in TMEM, double buffered) -> tcgen05.ld epilogue with fused bias / GELU / ReLU / gelu' / residual.
+// Batched bf16 GEMM for sm_90a: TMA -> 128B-swizzled shared memory -> wgmma (fp32 accumulators in registers) ->
+// register epilogue with fused bias / GELU / ReLU / gelu' / dropout / residual.
 //
-// Persistent, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane),
-// warps 2..9 = epilogue (warp w owns TMEM lanes 32*(w%4) .. +31, two warps per lane quarter). One CTA per SM.
+// Persistent, warp-specialised: warps 0..7 = two consumer warpgroups (warpgroup c owns accumulator rows
+// 64 c .. 64 c + 63 of the tile, issues its wgmma and runs its own epilogue), warp 8 = TMA producer (one lane).
+// One CTA per SM; the producer runs ahead through a ring of shared-memory stages, so the next tile's operands arrive
+// while the consumers are in the epilogue of the current one.
 //
-// Tile: 128 (M) x block_n (N, runtime, <=256) x 64 (K) per pipeline stage. Operands may be K-major or
-// MN-major (transposed in memory), which gives all of  X*W^T (forward), dY*W (dX) and dY^T*X (dW)
+// Tile: 128 (M) x BN (N, 64 or 128) x 64 (K) per pipeline stage. Operands may be K-major or MN-major (transposed in
+// memory; wgmma reads either from shared memory), which gives all of  X*W^T (forward), dY*W (dX) and dY^T*X (dW)
 // and the batched attention products without any transposition pass over HBM.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -25,14 +27,9 @@ namespace bb {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int NUM_THREADS = 320;  // 1 TMA warp + 1 MMA warp + 8 epilogue warps
+constexpr int NUM_THREADS = 288;  // 2 consumer warpgroups + 1 producer warp
 constexpr int MAX_STAGES = 8;
-constexpr int TMEM_COLS = 512;
-constexpr int STAGE_ROW_BYTES = 144;                     // 128 B of a row + 16 B pad (conflict-free 16-byte accesses)
-constexpr int STAGE_WARP_BYTES = 16 * STAGE_ROW_BYTES;   // 16 rows per pass
-constexpr int STAGE_BYTES = 8 * STAGE_WARP_BYTES;        // 18 KB for the 8 epilogue warps
 
 struct GemmKParams {
   int M, N, K;
@@ -56,7 +53,6 @@ struct GemmKParams {
   unsigned long long drop_seed;
   unsigned int drop_thresh;
   float drop_scale;
-  int staged;         // coalesced epilogue stores through the smem staging area (BB_GEMM_STAGED=0 turns it off)
   int fast_gelu;      // experiment: Abramowitz-Stegun erf on approximate MUFU ops instead of erff()
   long long* trace;   // debug: per CTA and local tile 4 globaltimer stamps (mma start/end, epilogue start/end) or null
   unsigned long long* prof;   // measurement: [0] = min over CTAs of the start stamp, [1] = max of the end stamp, or null
@@ -88,507 +84,253 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmKParams& p, int tile)
 
 __device__ __forceinline__ float bf2f(__nv_bfloat16 v) { return __bfloat162float(v); }
 
-// CTAS = 1: one CTA per 128 x block_n tile.  CTAS = 2: a CTA pair (cluster of 2 on one TPC) per 256 x block_n tile with
-// tcgen05.mma.cta_group::2 -- each CTA stages its 128 rows of A and half of the B tile, the leader issues the MMAs,
-// every CTA runs the epilogue of its own 128 accumulator rows.
-// EPI selects the epilogue at compile time: 0 = every feature (activation, second output, gelu'/relu' multiply,
-// dropout, residual add, any store), 1 = plain (alpha, optional bias, bf16 or fp32 store), 2 = fp32 atomic accumulate
-// (split-K weight gradients).  The specialised variants drop the operand-prefetch registers and feature branches of
-// the generic path: a per-tile timestamp trace showed the generic epilogue at ~7 us per 128x256 tile against a 4.7 us
-// mainloop at K = 768, i.e. every K = 768 product was epilogue-bound.
-template <int CTAS, int EPI>
+// Epilogue of two adjacent output columns (col, col + 1) of one row; col is even.  EPI selects the features at compile
+// time: 0 = every feature (activation, second output, gelu'/relu' multiply, dropout, residual add, any store),
+// 1 = plain (alpha, optional bias, bf16 or fp32 store), 2 = fp32 atomic accumulate (split-K weight gradients).
+template <int EPI>
+__device__ __forceinline__ void epi_pair(const GemmKParams& p, long long row_off, int col, float v0, float v1,
+                                         bool add_bias) {
+  const bool two = col + 1 < p.N;
+  const bool vec = two && p.vec_ok;
+  v0 *= p.alpha;
+  v1 *= p.alpha;
+  if (add_bias) {
+    v0 += __ldg(p.bias + col);
+    if (two) v1 += __ldg(p.bias + col + 1);
+  }
+  const long long off = row_off + col;
+  const bool out_f32 = EPI == 2 ? true : (p.out_f32 != 0);
+  const bool atomic = EPI == 2 ? true : (EPI == 1 ? false : p.atomic != 0);
+  if constexpr (EPI == 0) {
+    if (p.aux_out != nullptr) {
+      if (vec) *reinterpret_cast<__nv_bfloat162*>(p.aux_out + off) = __floats2bfloat162_rn(v0, v1);
+      else {
+        p.aux_out[off] = __float2bfloat16(v0);
+        if (two) p.aux_out[off + 1] = __float2bfloat16(v1);
+      }
+    }
+    if (p.act == 1) {
+      if (p.fast_gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+      else { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+    } else if (p.act == 2) {
+      v0 = fmaxf(v0, 0.0f);
+      v1 = fmaxf(v1, 0.0f);
+    }
+    if (p.epi_mul != 0) {
+      float a0, a1 = 0.0f;
+      if (vec) {
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.aux_in + off));
+        a0 = a.x;
+        a1 = a.y;
+      } else {
+        a0 = bf2f(p.aux_in[off]);
+        if (two) a1 = bf2f(p.aux_in[off + 1]);
+      }
+      if (p.epi_mul == 1) {
+        if (p.fast_gelu) { v0 *= dgelu_fast(a0); v1 *= dgelu_fast(a1); }
+        else { v0 *= dgelu_erf(a0); v1 *= dgelu_erf(a1); }
+      } else {
+        v0 = a0 > 0.0f ? v0 : 0.0f;
+        v1 = a1 > 0.0f ? v1 : 0.0f;
+      }
+    }
+    if (p.drop_thresh != 0) {
+      v0 = drop_keep(p.drop_seed, (uint64_t)off, p.drop_thresh) ? v0 * p.drop_scale : 0.0f;
+      v1 = drop_keep(p.drop_seed, (uint64_t)(off + 1), p.drop_thresh) ? v1 * p.drop_scale : 0.0f;
+    }
+    if (p.add_in != nullptr) {
+      if (vec) {
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.add_in + off));
+        v0 += a.x;
+        v1 += a.y;
+      } else {
+        v0 += bf2f(p.add_in[off]);
+        if (two) v1 += bf2f(p.add_in[off + 1]);
+      }
+    }
+  }
+  if (out_f32) {
+    float* D = reinterpret_cast<float*>(p.D) + off;
+    if (atomic) {
+      if (vec) {
+        atomicAdd(reinterpret_cast<float2*>(D), make_float2(v0, v1));
+      } else {
+        atomicAdd(D, v0);
+        if (two) atomicAdd(D + 1, v1);
+      }
+    } else if (vec) {
+      *reinterpret_cast<float2*>(D) = make_float2(v0, v1);
+    } else {
+      D[0] = v0;
+      if (two) D[1] = v1;
+    }
+  } else {
+    __nv_bfloat16* D = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
+    if (vec) *reinterpret_cast<__nv_bfloat162*>(D) = __floats2bfloat162_rn(v0, v1);
+    else {
+      D[0] = __float2bfloat16(v0);
+      if (two) D[1] = __float2bfloat16(v1);
+    }
+  }
+}
+
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (BN == 64) wgmma_m64n64_ss<TA, TB>(acc, da, db, scale_d);
+  else wgmma_m64n128_ss<TA, TB>(acc, da, db, scale_d);
+}
+
+// k-blocks [kb0, kb1) of one tile into this warpgroup's accumulators.  TA / TB (operand MN-major) are template
+// parameters so that the whole loop is free of branches around the asynchronous MMAs.
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint8_t* smem, int stage_bytes, uint64_t* full_bar,
+                                         uint64_t* empty_bar, int stages, int& stage, uint32_t& phase, int kb0, int kb1,
+                                         int wg, int lane) {
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes) + wg * 8192;
+    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + A_STAGE_BYTES;
+    fence_regs(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BLOCK_K / 16; ++k) {
+      const uint64_t da = TA ? wgmma_desc(sa + k * 2048, 8192, 1024) : wgmma_desc(sa + k * 32, 16, 1024);
+      const uint64_t db = TB ? wgmma_desc(sb + k * 2048, 8192, 1024) : wgmma_desc(sb + k * 32, 16, 1024);
+      wgmma_tile<BN, TA, TB>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    fence_regs(acc);
+    // at most the group just issued is in flight: the previous stage has been read and can be refilled
+    wgmma_wait<1>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+template <int BN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmKParams p, int total_tiles) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment for SWIZZLE_128B atoms (the dynamic smem base offset is the same in both CTAs of a pair)
+  // 1024-byte alignment for SWIZZLE_128B atoms
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int rank = CTAS == 2 ? (int)cluster_ctarank() : 0;
-  const int tile0 = blockIdx.x / CTAS, tile_step = gridDim.x / CTAS;
-  const int bn_local = p.block_n / CTAS;                 // B rows staged by this CTA
-  const int b_stage_bytes = bn_local * BLOCK_K * 2;
-  const int stage_bytes = A_STAGE_BYTES + b_stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
+  constexpr int B_STAGE_BYTES = BN * BLOCK_K * 2;
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tmem_full = empty_bar + MAX_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* sbias = reinterpret_cast<float*>(smem + p.stages * stage_bytes + 512);  // [2][256], one per accumulator
-  uint8_t* sstage = smem + p.stages * stage_bytes + 512 + 2048;                   // epilogue store staging, 8 warps
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8 * CTAS);   // the leader's MMA thread waits for the epilogue warps of both CTAs
+      mbar_init(&empty_bar[i], 8);   // lane 0 of every consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (CTAS == 2) {
-      tmem_alloc_2sm(tmem_ptr_smem, TMEM_COLS);
-      tmem_relinquish_2sm();
-    } else {
-      tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (CTAS == 2) cluster_sync_all();   // the peer's barriers must exist before TMA / commits signal them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // Everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the previous kernel's tail;
-  // from here on global memory is read and written.
+  __syncthreads();
+  // Everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail; from here on global
+  // memory is read and written.
   pdl_wait();
   pdl_trigger();
   if (p.prof && threadIdx.x == 0) atomicMin(p.prof, (unsigned long long)gtimer());
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      auto load = [&](void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-        if (CTAS == 2) tma_load_4d_2sm(dst, m, bar, c0, c1, c2, c3);   // completes on the LEADER's barrier
-        else tma_load_4d(dst, m, bar, c0, c1, c2, c3);
-      };
-      for (int tile = tile0; tile < total_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile(p, tile);
         const int kb0 = t.split * p.kb_per_split;
         const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        const int m0 = (t.m_tile * CTAS + rank) * BLOCK_M;
-        const int n0 = t.n_tile * p.block_n + rank * bn_local;
+        const int m0 = t.m_tile * BLOCK_M;
+        const int n0 = t.n_tile * BN;
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * stage_bytes;
+          mbar_wait_relaxed(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
           uint8_t* sb = sa + A_STAGE_BYTES;
-          if (rank == 0) mbar_expect_tx(&full_bar[stage], stage_bytes * CTAS);
+          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
           const int k0 = kb * BLOCK_K;
           if (!p.a_mn) {
-            load(sa, &tmap_a, &full_bar[stage], k0, m0, t.b1, t.b2);
+            tma_load_4d(sa, &tmap_a, &full_bar[stage], k0, m0, t.b1, t.b2);
           } else {
-            load(sa, &tmap_a, &full_bar[stage], m0, k0, t.b1, t.b2);
-            load(sa + 8192, &tmap_a, &full_bar[stage], m0 + 64, k0, t.b1, t.b2);
+            tma_load_4d(sa, &tmap_a, &full_bar[stage], m0, k0, t.b1, t.b2);
+            tma_load_4d(sa + 8192, &tmap_a, &full_bar[stage], m0 + 64, k0, t.b1, t.b2);
           }
           if (!p.b_mn) {
-            load(sb, &tmap_b, &full_bar[stage], k0, n0, t.b1, t.b2);
+            tma_load_4d(sb, &tmap_b, &full_bar[stage], k0, n0, t.b1, t.b2);
           } else {
-            for (int j = 0; j < bn_local / 64; ++j)
-              load(sb + j * 8192, &tmap_b, &full_bar[stage], n0 + 64 * j, k0, t.b1, t.b2);
-          }
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = umma_idesc_bf16(BLOCK_M * CTAS, p.block_n, p.a_mn, p.b_mn);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = tile0; tile < total_tiles; tile += tile_step) {
-        const TileCoord t = decode_tile(p, tile);
-        const int kb0 = t.split * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const int lt = (tile - tile0) / tile_step;
-        if (p.trace && lt < 16) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 0] = gtimer();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sb = sa + A_STAGE_BYTES;
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint64_t da = p.a_mn ? umma_smem_desc(sa + k * 2048, 8192, 1024)
-                                       : umma_smem_desc(sa + k * 32, 16, 1024);
-            const uint64_t db = p.b_mn ? umma_smem_desc(sb + k * 2048, 8192, 1024)
-                                       : umma_smem_desc(sb + k * 32, 16, 1024);
-            if (CTAS == 2) umma_bf16_ss_2sm(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_bf16_ss(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
+            for (int j = 0; j < BN / 64; ++j)
+              tma_load_4d(sb + j * 8192, &tmap_b, &full_bar[stage], n0 + 64 * j, k0, t.b1, t.b2);
           }
-          // smem slot reusable once these MMAs retire (in both CTAs of a pair)
-          if (CTAS == 2) umma_commit_2sm(&empty_bar[stage]);
-          else umma_commit(&empty_bar[stage]);
           if (++stage == p.stages) {
             stage = 0;
             phase ^= 1;
           }
         }
-        // accumulator complete -> epilogue (of both CTAs)
-        if (CTAS == 2) umma_commit_2sm(&tmem_full[acc]);
-        else umma_commit(&tmem_full[acc]);
-        if (p.trace && lt < 16) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 1] = gtimer();   // issue done (not retired)
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
       }
     }
   } else {
-    // ------------------------------------------------------------------ epilogue (8 warps)
-    // warps 2..9: warp w owns TMEM lanes 32*(w%4)..+31 (hardware rule) and every other 16-column chunk of the
-    // tile (two warps per lane quarter).  Global epilogue operands (gelu'/relu' input, residual) of the NEXT chunk
-    // are prefetched into registers before the current chunk is processed, so their latency is off the critical path.
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const bool need_aux = EPI == 0 && p.epi_mul != 0;
-    const bool need_add = EPI == 0 && p.add_in != nullptr;
-    const bool has_aux_out = EPI == 0 && p.aux_out != nullptr;
-    const int act = EPI == 0 ? p.act : 0;
-    const unsigned int drop_thresh = EPI == 0 ? p.drop_thresh : 0u;
-    const bool out_f32 = EPI == 2 ? true : (p.out_f32 != 0);
-    const bool atomic = EPI == 2 ? true : (EPI == 1 ? false : p.atomic != 0);
-    for (int tile = tile0; tile < total_tiles; tile += tile_step) {
+    // ------------------------------------------------------------------ consumers: wgmma mainloop + epilogue
+    const int wg = warp >> 2;                       // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+    const int r0 = (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8 of the warpgroup's 64
+    const int cq = 2 * (lane & 3);                  // fragment column offset within each 8-column group
+    int stage = 0;
+    uint32_t phase = 0;
+    int lt = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
       const TileCoord t = decode_tile(p, tile);
-      const int row = (t.m_tile * CTAS + rank) * BLOCK_M + quarter * 32 + lane;
-      const int n0 = t.n_tile * p.block_n;
-      const bool row_ok = row < p.M;
-      const long long row_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2 + (long long)row * p.ldd;
+      const int kb0 = t.split * p.kb_per_split;
+      const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+      const bool stamp = p.trace && lt < 16 && threadIdx.x == 0;
+      if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 0] = gtimer();
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      switch (p.a_mn * 2 + p.b_mn) {
+        case 0: mainloop<BN, 0, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
+        case 1: mainloop<BN, 0, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
+        case 2: mainloop<BN, 1, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
+        default: mainloop<BN, 1, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
+      }
+      if (stamp) {
+        p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 1] = gtimer();
+        p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 2] = gtimer();
+      }
+      // ---- epilogue straight from the accumulator registers
+      const int n0 = t.n_tile * BN;
       const bool add_bias = p.bias != nullptr && t.split == 0;
-      if (p.bias != nullptr) {
-        // stage this tile's bias slice in shared memory (one coalesced read instead of dependent loads per chunk)
-        float* sb = sbias + acc * 256;
-        const int e = (warp - 2) * 32 + lane;  // 0..255
-        for (int i = e; i < p.block_n; i += 256) sb[i] = (n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.0f;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
-      // prefetch registers for the first chunk
-      uint4 pa[2], pd[2];
-      pa[0] = pa[1] = pd[0] = pd[1] = make_uint4(0, 0, 0, 0);
-      auto prefetch = [&](int c) {
-        const int col0 = n0 + c;
-        if (c < p.block_n && row_ok && p.vec_ok && col0 + 16 <= p.N) {
-          const long long off = row_off + col0;
-          if (need_aux) {
-            const uint4* src = reinterpret_cast<const uint4*>(p.aux_in + off);
-            pa[0] = __ldg(src);
-            pa[1] = __ldg(src + 1);
-          }
-          if (need_add) {
-            const uint4* src = reinterpret_cast<const uint4*>(p.add_in + off);
-            pd[0] = __ldg(src);
-            pd[1] = __ldg(src + 1);
-          }
-        }
-      };
-      prefetch(half * 16);
-
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const int lt = (tile - tile0) / tile_step;
-      if (p.trace && lt < 16 && warp == 2 && lane == 0) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 2] = gtimer();
-      const uint32_t taddr = tmem_base + (uint32_t(quarter * 32) << 16) + acc * 256;
-      if constexpr (EPI != 0) {
-        // Specialised epilogues: 32-column TMEM loads, the next one in flight while the current 32 columns are
-        // scaled / biased / converted / stored.  Warp `half` takes every other 32-column chunk.
-        auto emit = [&](const uint32_t* r, const int c) {   // 16 columns starting at tile column c
-          const int col0 = n0 + c;
-          if (c >= p.block_n || col0 >= p.N || !row_ok) return;
-          float v[16];
+      const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]) * p.alpha;
-          if (add_bias) {
-            const float4* sb4 = reinterpret_cast<const float4*>(sbias + acc * 256 + c);
+      for (int h = 0; h < 2; ++h) {
+        const int row = t.m_tile * BLOCK_M + wg * 64 + r0 + 8 * h;
+        if (row >= p.M) continue;
+        const long long row_off = batch_off + (long long)row * p.ldd;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 bv = sb4[i];
-              v[4 * i] += bv.x;
-              v[4 * i + 1] += bv.y;
-              v[4 * i + 2] += bv.z;
-              v[4 * i + 3] += bv.w;
-            }
-          }
-          const bool full = (col0 + 16 <= p.N) && p.vec_ok;
-          const long long off = row_off + col0;
-          if (out_f32) {
-            float* D = reinterpret_cast<float*>(p.D) + off;
-            if (atomic) {
-              if (full) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(D + 4 * i), "f"(v[4 * i]),
-                               "f"(v[4 * i + 1]), "f"(v[4 * i + 2]), "f"(v[4 * i + 3])
-                               : "memory");
-              } else {
-                for (int i = 0; i < 16; ++i)
-                  if (col0 + i < p.N) atomicAdd(D + i, v[i]);
-              }
-            } else if (full) {
-              float4* dst = reinterpret_cast<float4*>(D);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) dst[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-            } else {
-              for (int i = 0; i < 16; ++i)
-                if (col0 + i < p.N) D[i] = v[i];
-            }
-          } else {
-            __nv_bfloat16* D = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
-            if (full) {
-              __align__(16) __nv_bfloat162 h[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) h[i] = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-              uint4* dst = reinterpret_cast<uint4*>(D);
-              dst[0] = reinterpret_cast<uint4*>(h)[0];
-              dst[1] = reinterpret_cast<uint4*>(h)[1];
-            } else {
-              for (int i = 0; i < 16; ++i)
-                if (col0 + i < p.N) D[i] = __float2bfloat16(v[i]);
-            }
-          }
-        };
-        // Slabs of 128 output bytes per row (64 bf16 or 32 fp32 columns); warp `half` takes every other slab.
-        // A lane owns one ROW of the accumulator, so storing straight from registers makes every store instruction
-        // touch 32 different 128-byte lines with 16 bytes each (the trace showed the epilogue bound by exactly that:
-        // ~6 us per 128x256 tile against a 4.7 us mainloop).  Each slab therefore goes through a per-warp shared
-        // memory staging area (16 rows x 144 B, two passes) and leaves as full 128-byte row segments: 4 lines per
-        // store instruction instead of 32.
-        const int W = out_f32 ? 32 : 64;
-        uint8_t* stg = sstage + (warp - 2) * STAGE_WARP_BYTES;
-        const int tile_row0 = (t.m_tile * CTAS + rank) * BLOCK_M + quarter * 32;
-        const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
-        for (int c = half * W; c < p.block_n; c += 2 * W) {
-          const int col0 = n0 + c;
-          if (col0 >= p.N) break;   // warp-uniform
-          uint32_t r[64];
-          {
-            uint32_t(&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-            uint32_t(&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-            tmem_ld32(taddr + c, r0);
-            if (!out_f32) {
-              tmem_ld32(taddr + c + 32, r1);
-              tmem_ld_wait32(r1);
-            }
-            tmem_ld_wait32(r0);
-          }
-          if (!(p.staged && p.vec_ok && col0 + W <= p.N && c + W <= p.block_n)) {   // ragged slab: direct stores
-            for (int k = 0; k < W / 16; ++k) emit(r + 16 * k, c + 16 * k);
-            continue;
-          }
-          uint4 pk[8];
-          if (out_f32) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 v = make_float4(__uint_as_float(r[4 * j]) * p.alpha, __uint_as_float(r[4 * j + 1]) * p.alpha,
-                                     __uint_as_float(r[4 * j + 2]) * p.alpha, __uint_as_float(r[4 * j + 3]) * p.alpha);
-              if (add_bias) {
-                const float4 bv = *reinterpret_cast<const float4*>(sbias + acc * 256 + c + 4 * j);
-                v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-              }
-              pk[j] = *reinterpret_cast<uint4*>(&v);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float v[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[8 * j + i]) * p.alpha;
-              if (add_bias) {
-                const float4 b0 = *reinterpret_cast<const float4*>(sbias + acc * 256 + c + 8 * j);
-                const float4 b1 = *reinterpret_cast<const float4*>(sbias + acc * 256 + c + 8 * j + 4);
-                v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-                v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
-              }
-              __nv_bfloat162 h0 = __floats2bfloat162_rn(v[0], v[1]), h1 = __floats2bfloat162_rn(v[2], v[3]);
-              __nv_bfloat162 h2 = __floats2bfloat162_rn(v[4], v[5]), h3 = __floats2bfloat162_rn(v[6], v[7]);
-              pk[j] = make_uint4(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1),
-                                 *reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
-            }
-          }
-          uint8_t* gbase = reinterpret_cast<uint8_t*>(p.D) + (batch_off + col0) * (out_f32 ? 4 : 2);
-          const long long row_bytes = p.ldd * (out_f32 ? 4 : 2);
-#pragma unroll
-          for (int pass = 0; pass < 2; ++pass) {
-            if ((lane >> 4) == pass) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) *reinterpret_cast<uint4*>(stg + (lane & 15) * STAGE_ROW_BYTES + j * 16) = pk[j];
-            }
-            __syncwarp();
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int rr = k * 4 + (lane >> 3), ch = lane & 7;
-              const uint4 val = *reinterpret_cast<const uint4*>(stg + rr * STAGE_ROW_BYTES + ch * 16);
-              const int grow = tile_row0 + pass * 16 + rr;
-              if (grow < p.M) {
-                uint8_t* dst = gbase + grow * row_bytes + ch * 16;
-                if (atomic) {
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(__uint_as_float(val.x)),
-                               "f"(__uint_as_float(val.y)), "f"(__uint_as_float(val.z)), "f"(__uint_as_float(val.w))
-                               : "memory");
-                } else {
-                  *reinterpret_cast<uint4*>(dst) = val;
-                }
-              }
-            }
-            __syncwarp();
-          }
-        }
-      } else
-      for (int c = half * 16; c < p.block_n; c += 32) {
-        const int col0 = n0 + c;
-        if (col0 >= p.N) break;  // warp-uniform
-        uint32_t r[16];
-        tmem_ld16(taddr + c, r);
-        // operands of this chunk (prefetched) -> locals, then start fetching the next chunk's
-        __align__(16) __nv_bfloat16 ha[16], hd[16];
-        reinterpret_cast<uint4*>(ha)[0] = pa[0];
-        reinterpret_cast<uint4*>(ha)[1] = pa[1];
-        reinterpret_cast<uint4*>(hd)[0] = pd[0];
-        reinterpret_cast<uint4*>(hd)[1] = pd[1];
-        prefetch(c + 32);
-        tmem_ld_wait();
-        if (!row_ok) continue;
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]) * p.alpha;
-        const bool full = (col0 + 16 <= p.N);
-        if (add_bias) {
-          const float4* sb4 = reinterpret_cast<const float4*>(sbias + acc * 256 + c);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 bv = sb4[i];
-            v[4 * i] += bv.x;
-            v[4 * i + 1] += bv.y;
-            v[4 * i + 2] += bv.z;
-            v[4 * i + 3] += bv.w;
-          }
-        }
-        const long long off = row_off + col0;
-        if (has_aux_out) {
-          if (full && p.vec_ok) {
-            __align__(16) __nv_bfloat162 h[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) h[i] = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-            uint4* dst = reinterpret_cast<uint4*>(p.aux_out + off);
-            dst[0] = reinterpret_cast<uint4*>(h)[0];
-            dst[1] = reinterpret_cast<uint4*>(h)[1];
-          } else {
-            for (int i = 0; i < 16; ++i)
-              if (col0 + i < p.N) p.aux_out[off + i] = __float2bfloat16(v[i]);
-          }
-        }
-        if (act == 1) {
-          if (p.fast_gelu) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = gelu_fast(v[i]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = gelu_erf(v[i]);
-          }
-        } else if (act == 2) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.0f);
-        }
-        if (need_aux) {
-          float a[16];
-          if (full && p.vec_ok) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) a[i] = bf2f(ha[i]);
-          } else {
-            for (int i = 0; i < 16; ++i) a[i] = (col0 + i < p.N) ? bf2f(p.aux_in[off + i]) : 0.0f;
-          }
-          if (p.epi_mul == 1) {
-            if (p.fast_gelu) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] *= dgelu_fast(a[i]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] *= dgelu_erf(a[i]);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = a[i] > 0.0f ? v[i] : 0.0f;
-          }
-        }
-        if (drop_thresh != 0) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            v[i] = drop_keep(p.drop_seed, (uint64_t)(off + i), drop_thresh) ? v[i] * p.drop_scale : 0.0f;
-        }
-        if (need_add) {
-          if (full && p.vec_ok) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += bf2f(hd[i]);
-          } else {
-            for (int i = 0; i < 16; ++i)
-              if (col0 + i < p.N) v[i] += bf2f(p.add_in[off + i]);
-          }
-        }
-        if (out_f32) {
-          float* D = reinterpret_cast<float*>(p.D) + off;
-          if (atomic) {
-            if (full && p.vec_ok) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(D + 4 * i), "f"(v[4 * i]),
-                             "f"(v[4 * i + 1]), "f"(v[4 * i + 2]), "f"(v[4 * i + 3])
-                             : "memory");
-            } else {
-              for (int i = 0; i < 16; ++i)
-                if (col0 + i < p.N) atomicAdd(D + i, v[i]);
-            }
-          } else if (full && p.vec_ok) {
-            float4* dst = reinterpret_cast<float4*>(D);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) dst[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          } else {
-            for (int i = 0; i < 16; ++i)
-              if (col0 + i < p.N) D[i] = v[i];
-          }
-        } else {
-          __nv_bfloat16* D = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
-          if (full && p.vec_ok) {
-            __align__(16) __nv_bfloat162 h[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) h[i] = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-            uint4* dst = reinterpret_cast<uint4*>(D);
-            dst[0] = reinterpret_cast<uint4*>(h)[0];
-            dst[1] = reinterpret_cast<uint4*>(h)[1];
-          } else {
-            for (int i = 0; i < 16; ++i)
-              if (col0 + i < p.N) D[i] = __float2bfloat16(v[i]);
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + cq;
+          if (col < p.N) epi_pair<EPI>(p, row_off, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], add_bias);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (p.trace && lt < 16 && warp == 2 && lane == 0) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 3] = gtimer();
-      if (lane == 0) {
-        if (CTAS == 2) mbar_arrive_leader(&tmem_empty[acc]);
-        else mbar_arrive(&tmem_empty[acc]);
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 3] = gtimer();
     }
   }
 
-  tc_fence_before();
-  if (CTAS == 2) cluster_sync_all();   // the leader's MMAs read the peer's smem and write its TMEM until the very end
-  else __syncthreads();
+  __syncthreads();
   if (p.prof && threadIdx.x == 0) atomicMax(p.prof + 1, (unsigned long long)gtimer());
-  if (warp == 2) {
-    tc_fence_after();
-    if (CTAS == 2) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------------ host side
@@ -691,7 +433,6 @@ static size_t g_prof_cap = 0;
 static long long* g_trace = nullptr;   // bb_gemm_trace(): device buffer of (grid x 16 x 4) timestamps, debug only
 static int g_num_sms = 0;
 static int g_smem_optin = 0;
-
 static int init_device_info() {
   if (g_num_sms) return 0;
   int dev = 0;
@@ -702,45 +443,10 @@ static int init_device_info() {
   auto set = [&](auto kernel) {
     ok = ok && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) == cudaSuccess;
   };
-  set(gemm_tc_kernel<1, 0>); set(gemm_tc_kernel<1, 1>); set(gemm_tc_kernel<1, 2>);
-  set(gemm_tc_kernel<2, 0>); set(gemm_tc_kernel<2, 1>); set(gemm_tc_kernel<2, 2>);
+  set(gemm_tc_kernel<64, 0>); set(gemm_tc_kernel<64, 1>); set(gemm_tc_kernel<64, 2>);
+  set(gemm_tc_kernel<128, 0>); set(gemm_tc_kernel<128, 1>); set(gemm_tc_kernel<128, 2>);
   if (!ok) return set_error("cudaFuncSetAttribute(max dynamic smem) failed for gemm_tc_kernel");
   return 0;
-}
-
-// number of CTA pairs that can be resident at once (GPCs with an odd SM count leave an SM without a partner)
-static int max_pairs() {
-  static int v = -1;
-  if (v < 0) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(g_num_sms / 2 * 2);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = g_smem_optin;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<2, 0>, &cfg) != cudaSuccess || n <= 0) {
-      cudaGetLastError();
-      n = g_num_sms / 2;
-    }
-    v = n < g_num_sms / 2 ? n : g_num_sms / 2;
-  }
-  return v;
-}
-
-// BB_GEMM_2CTA: 0 = single-CTA tiles only, 1 (default) = CTA pairs wherever the shape allows
-static int two_cta_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("BB_GEMM_2CTA");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
 }
 
 }  // namespace bb
@@ -763,6 +469,8 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   if (atomic && !a->out_f32) return set_error("bb_gemm_bf16: accumulate / split_k need fp32 output");
   if (atomic && (a->act || a->epi_mul || a->aux_out || a->add_in || a->drop_thresh))
     return set_error("bb_gemm_bf16: accumulate / split_k cannot be combined with a non-linear epilogue");
+  if (a->block_n > 0 && (a->block_n < 16 || a->block_n > 256 || a->block_n % 16 != 0 || (a->b_mn && a->block_n % 64 != 0)))
+    return set_error("bb_gemm_bf16: invalid block_n");
 
   GemmKParams p;
   memset(&p, 0, sizeof(p));
@@ -773,37 +481,18 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   p.nb2 = nb2;
   p.a_mn = a->a_mn ? 1 : 0;
   p.b_mn = a->b_mn ? 1 : 0;
-  // CTA pairs (256-row tiles, +7..11 % on machine-filling problems) only when the single-CTA tiling would need at
-  // least two full rounds of the machine: a pair costs a cluster launch plus two cluster barriers, which the 10-30 us
-  // language-encoder products do not amortise (measured).  BB_GEMM_2CTA=2 forces pairs wherever legal (tests).
-  int ctas = 1;
-  if (two_cta_mode() && a->M > BLOCK_M) {
-    const long long t1 = (long long)((a->M + BLOCK_M - 1) / BLOCK_M) * ((a->N + 255) / 256) * nb1 * nb2 * split_k_req;
-    if (two_cta_mode() >= 2 || t1 >= 2LL * g_num_sms) ctas = 2;
-  }
-  p.m_tiles = (a->M + BLOCK_M * ctas - 1) / (BLOCK_M * ctas);
-  // N tile
-  int bn = a->block_n;
-  if (bn <= 0) {
-    const int gran = p.b_mn ? 64 : 16;
-    if (a->N <= 128) {
-      bn = ((a->N + gran - 1) / gran) * gran;  // one N tile
-    } else {
-      // The mainloop is latency-bound per k-block (measured ~0.5 us whatever the tile width), so the cost of a
-      // launch is ~ rounds x k-blocks x t(bn) with t(256) ~ 1.3 t(128): pick the width with fewer weighted rounds.
-      const long long per = (long long)p.m_tiles * nb1 * nb2 * split_k_req;
-      const int n256 = (a->N + 255) / 256, n128 = (a->N + 127) / 128;
-      const int units = ctas == 2 ? max_pairs() : g_num_sms;
-      const long long r256 = (per * n256 + units - 1) / units, r128 = (per * n128 + units - 1) / units;
-      bn = (13 * r256 <= 10 * r128) ? 256 : 128;
-      if (a->N <= 256 && bn == 256) bn = ((a->N + gran - 1) / gran) * gran;
-    }
-  }
-  if (bn < 16 || bn > 256 || bn % 16 != 0 || (p.b_mn && bn % 64 != 0))
-    return set_error("bb_gemm_bf16: invalid block_n");
-  if (ctas == 2 && (bn % 32 != 0 || (p.b_mn && bn % 128 != 0))) {   // each CTA stages bn/2 rows of B
-    ctas = 1;
-    p.m_tiles = (a->M + BLOCK_M - 1) / BLOCK_M;
+  p.m_tiles = (a->M + BLOCK_M - 1) / BLOCK_M;
+  // N tile: the kernel is built for 64- and 128-wide tiles (a 64 x 128 fp32 accumulator is 64 registers per thread).
+  // A requested block_n is a width hint: <= 64 selects the narrow tile.  Otherwise narrow tiles are used for narrow
+  // products and whenever 128-wide tiles would leave more than half of the SMs idle.
+  int bn;
+  if (a->block_n > 0) {
+    bn = a->block_n <= 64 ? 64 : 128;
+  } else if (a->N <= 64) {
+    bn = 64;
+  } else {
+    const long long t128 = (long long)p.m_tiles * ((a->N + 127) / 128) * nb1 * nb2 * split_k_req;
+    bn = 2 * t128 < g_num_sms ? 64 : 128;
   }
   p.block_n = bn;
   p.n_tiles = (a->N + bn - 1) / bn;
@@ -836,17 +525,11 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
       fg = (e_ && e_[0] == '1') ? 1 : 0;
     }
     p.fast_gelu = fg;
-    static int st = -1;
-    if (st < 0) {
-      const char* e_ = getenv("BB_GEMM_STAGED");
-      st = (e_ && e_[0] == '0') ? 0 : 1;
-    }
-    p.staged = st;
   }
   if (p.epi_mul && !p.aux_in) return set_error("bb_gemm_bf16: epi_mul needs aux_in");
-  // vector epilogue only when every row segment of 16 outputs is 16-byte aligned (for bf16: 8 elements)
+  // paired (2-element) epilogue accesses only when every row segment is suitably aligned
   {
-    const int al = 8;  // elements; covers bf16 (16 B) and f32 (32 B)
+    const int al = 8;  // elements
     bool ok = (a->ldd % al == 0) && (a->d_s1 % al == 0) && (a->d_s2 % al == 0);
     ok = ok && ((reinterpret_cast<uintptr_t>(a->D) & 15) == 0);
     if (a->aux_out) ok = ok && ((reinterpret_cast<uintptr_t>(a->aux_out) & 15) == 0);
@@ -855,9 +538,7 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
     p.vec_ok = ok ? 1 : 0;
   }
 
-  // epilogue variant (BB_GEMM_EPI=0 forces the generic one, for A/B runs).  A staged (coalesced) variant of the
-  // GELU / gelu' epilogues was measured in round 2 (profiles/r02_selftest_gelu_staged.log): correct but slower than
-  // the direct stores (perf_ffn1 448 vs 567 TFLOP/s) and removed.
+  // epilogue variant (BB_GEMM_EPI=0 forces the generic one, for A/B runs)
   static const int epi_mode = [] {
     const char* e_ = getenv("BB_GEMM_EPI");
     return (e_ && e_[0] == '0') ? 0 : 1;
@@ -865,10 +546,9 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   int epi = 0;
   const bool featureless = !p.act && !p.aux_out && !p.epi_mul && !p.add_in && !p.drop_thresh;
   if (epi_mode && featureless) epi = p.atomic ? (p.bias ? 0 : 2) : 1;
-  const int stage_reserve = STAGE_BYTES;
 
-  const int stage_bytes = A_STAGE_BYTES + (bn / ctas) * BLOCK_K * 2;
-  int stages = (g_smem_optin - 1024 - 512 - 2048 - stage_reserve) / stage_bytes;
+  const int stage_bytes = A_STAGE_BYTES + bn * BLOCK_K * 2;
+  int stages = (g_smem_optin - 1024 - 256) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   {
     static int env_stages = -1;  // BB_GEMM_STAGES: pipeline-depth experiments only
@@ -880,21 +560,20 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   }
   if (stages < 2) return set_error("bb_gemm_bf16: not enough shared memory for 2 stages");
   p.stages = stages;
-  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + 512 + 2048 + stage_reserve;
+  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + 256;
 
   CUtensorMap ta, tb;
   int e;
   if (!p.a_mn) e = make_map(&ta, a->A, a->K, a->M, nb1, nb2, a->lda, a->a_s1, a->a_s2, BLOCK_M);
   else e = make_map(&ta, a->A, a->M, a->K, nb1, nb2, a->lda, a->a_s1, a->a_s2, BLOCK_K);
   if (e) return e;
-  if (!p.b_mn) e = make_map(&tb, a->B, a->K, a->N, nb1, nb2, a->ldb, a->b_s1, a->b_s2, bn / ctas);
+  if (!p.b_mn) e = make_map(&tb, a->B, a->K, a->N, nb1, nb2, a->ldb, a->b_s1, a->b_s2, bn);
   else e = make_map(&tb, a->B, a->N, a->K, nb1, nb2, a->ldb, a->b_s1, a->b_s2, BLOCK_K);
   if (e) return e;
 
   const long long total = (long long)p.m_tiles * p.n_tiles * nb1 * nb2 * p.split_k;
   if (total > 0x7fffffffLL) return set_error("bb_gemm_bf16: too many tiles");
-  const int units = ctas == 2 ? max_pairs() : g_num_sms;
-  const int grid = (total < units ? (int)total : units) * ctas;
+  const int grid = total < g_num_sms ? (int)total : g_num_sms;
   if (g_prof_on && g_prof_buf && g_prof_used < g_prof_cap) {
     if (g_prof_used == g_prof.size()) g_prof.push_back(ProfRec());
     ProfRec* rec = &g_prof[g_prof_used];
@@ -903,13 +582,16 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
     p.prof = g_prof_buf + 2 * g_prof_used;
     ++g_prof_used;
   }
-  auto go = [&](auto k1, auto k2) {
-    if (ctas == 2) bb::launch_pdl_cluster(k2, grid, NUM_THREADS, smem_bytes, stream, 2, ta, tb, p, (int)total);
-    else bb::launch_pdl(k1, grid, NUM_THREADS, smem_bytes, stream, ta, tb, p, (int)total);
-  };
-  if (epi == 1) go(gemm_tc_kernel<1, 1>, gemm_tc_kernel<2, 1>);
-  else if (epi == 2) go(gemm_tc_kernel<1, 2>, gemm_tc_kernel<2, 2>);
-  else go(gemm_tc_kernel<1, 0>, gemm_tc_kernel<2, 0>);
+  auto go = [&](auto kernel) { bb::launch_pdl(kernel, grid, NUM_THREADS, smem_bytes, stream, ta, tb, p, (int)total); };
+  if (bn == 64) {
+    if (epi == 1) go(gemm_tc_kernel<64, 1>);
+    else if (epi == 2) go(gemm_tc_kernel<64, 2>);
+    else go(gemm_tc_kernel<64, 0>);
+  } else {
+    if (epi == 1) go(gemm_tc_kernel<128, 1>);
+    else if (epi == 2) go(gemm_tc_kernel<128, 2>);
+    else go(gemm_tc_kernel<128, 0>);
+  }
   count_launch();
   return check_launch("gemm_tc_kernel");
 }

@@ -130,7 +130,7 @@ static int num_sms() {     // split-K factor of the weight-gradient products: fi
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;   // H100 SXM
   }
   return n;
 }
@@ -138,8 +138,10 @@ static int num_sms() {     // split-K factor of the weight-gradient products: fi
 static int lin_bwd_dw(const void* dy, const void* x, float* out, int64_t M, int N, int Kd, void* stream) {
   bb_gemm_args g;
   memset(&g, 0, sizeof(g));
+  // same tiling rule as blocks.lin_bwd_dw: 128-wide tiles when they fill half the SMs, else 64-wide, then split the
+  // token dimension until about one CTA per SM, keeping >= 8 k-blocks per split
   const int m_t = (N + 127) / 128;
-  int bn = (m_t * ((Kd + 255) / 256) >= 74) ? 256 : 128;
+  int bn = (m_t * ((Kd + 127) / 128) >= num_sms() / 2) ? 128 : 64;
   if (Kd <= bn) bn = 0;
   const int tiles = bn ? m_t * ((Kd + bn - 1) / bn) : m_t;
   const int64_t kb = (M + 63) / 64;

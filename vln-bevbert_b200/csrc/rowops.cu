@@ -1,4 +1,4 @@
-// HBM-bound row kernels for the BEVBert encoder stack on sm_100a: casts with dropout, fused
+// HBM-bound row kernels for the BEVBert encoder stack on sm_90a: casts with dropout, fused
 // (dropout + residual +) LayerNorm forward/backward, masked softmax forward/backward with the graph bias,
 // bias-gradient column sums, embedding sum / scatter, row gather / scatter-add and fused softmax
 // cross-entropy. One warp per row where rows are <= 1024 wide, 16-byte vector accesses, fp32 math,
@@ -794,7 +794,18 @@ softmax_xent_kernel(const float* __restrict__ logits, const int64_t* __restrict_
   }
 }
 
-static inline unsigned grid1d(long long n, int per_block, int cap = 148 * 16) {
+static int device_sms() {   // grid caps of the grid-strided kernels: the SM count of the device this library runs on
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+      n = 132;   // H100 SXM
+  }
+  return n;
+}
+static inline unsigned grid1d(long long n, int per_block, int cap = 0) {
+  if (cap <= 0) cap = device_sms() * 16;
   long long g = (n + per_block - 1) / per_block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -927,7 +938,7 @@ extern "C" int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x
   if (rows <= 0) return 0;
   if (H % 8 != 0 || H > LN_MAXCH * 256) return set_error("bb_layernorm_bwd: H must be a multiple of 8 and <= 1024");
   long long g = (rows + LN_WARPS - 1) / LN_WARPS;
-  if (g > 148) g = 148;   // one resident block per SM (233 registers), rows grid-strided
+  if (g > device_sms()) g = device_sms();   // one resident block per SM (233 registers), rows grid-strided
   const unsigned grid = (unsigned)g;
   const size_t ln_smem = (size_t)3 * LN_WARPS * H * sizeof(float);
 #define LN_BWD(DYT, XT, DXT, AT)                                                                                    \

@@ -1,7 +1,7 @@
 """Whole-step CUDA-graph replay for the pre-training loop: forward + backward (+ gradient all-reduce) + optimizer of one
 (task, batch-shape) is captured once and replayed, so a step costs the host one `cudaGraphLaunch` instead of ~600 kernel
-launches plus the Python block / autograd glue (the step is host-bound otherwise: ~14.7 ms per step on a B200 whatever the
-kernels do).
+launches plus the Python block / autograd glue (eager stepping spends that much host time per step whatever the kernels
+do).
 
 What makes a step replayable here:
   * inputs live in STATIC device tensors (the caller refills them in place, e.g. from pinned host memory on a copy
@@ -111,7 +111,7 @@ class GraphedTrainStep:
             # data-parallel: the graph holds forward + backward; the NCCL all-reduce and the optimizer run eagerly on the
             # gradients the graph left in its (static) arena.  Collectives stay out of the capture: a rank whose capture
             # failed would execute them while the others only record them, and capturing the chunked reductions on the
-            # communication stream faulted on B200 (round 2, N=2: illegal address at the first replay) -- not pursued.
+            # communication stream faulted in an earlier two-GPU experiment (illegal address at the first replay).
             ent["graph"].replay()
             self._after_backward_eager(ent)
             return ent["loss"]

@@ -82,7 +82,7 @@ def reset_launch_count():
 def gemm(a, b, out, M, N, K, lda, ldb, ldd, a_mn=False, b_mn=False, nb1=1, nb2=1, a_s=(0, 0), b_s=(0, 0),
          d_s=(0, 0), alpha=1.0, bias=None, act=ACT_NONE, aux_out=None, aux_in=None, epi_mul=EPI_NONE, add_in=None,
          accumulate=False, split_k=1, drop=(0, 0, 1.0), block_n=0):
-    """out = epi(alpha * A @ B^T) on tcgen05; a/b/out are base tensors (pointer = data_ptr()), strides in
+    """out = epi(alpha * A @ B^T) on wgmma; a/b/out are base tensors (pointer = data_ptr()), strides in
     elements.  out dtype bf16 or f32 decides the output type.  drop = (seed, thresh, scale)."""
     lib = _lib.load()
     _req(a, act_dtype(), "a")
@@ -117,7 +117,7 @@ _PROF_BUF = None
 
 
 def gemm_profile(enable: bool, capacity: int = 8192):
-    """Start / stop the library's per-launch GEMM timing: every tcgen05 GEMM launch stamps %globaltimer (first CTA
+    """Start / stop the library's per-launch GEMM timing: every wgmma GEMM launch stamps %globaltimer (first CTA
     start, last CTA end) into its slot of a device buffer -- no events between launches."""
     global _PROF_BUF
     lib = _lib.load()
@@ -254,7 +254,7 @@ def _flash_args(q, k, v, o, lse, B, H, nq, nk, ldq, ldk, ldv, ldo, kmask, bias, 
 
 
 def set_attn_tc(mode: int) -> int:
-    """0: mma.sync attention kernels only; 1: tcgen05 kernels for nk >= 64 (default); 2: tcgen05 wherever supported."""
+    """0: mma.sync attention kernels only; 1: wgmma kernels for nk >= 64 (default); 2: wgmma wherever supported."""
     return int(_lib.load().bb_set_attn_tc(int(mode)))
 
 

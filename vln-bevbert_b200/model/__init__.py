@@ -1,2 +1,2 @@
 """The reference's model class surface (pretrain_src/model/{vilmodel,pretrain_cmt,bev_utils,ops}.py) on the
-B200 kernels: same class names, constructor / forward signatures and state_dict keys."""
+H100 kernels: same class names, constructor / forward signatures and state_dict keys."""

@@ -1,4 +1,4 @@
-"""BEV lifting on the B200 kernels: same entry points as pretrain_src/model/bev_utils.py
+"""BEV lifting on the H100 kernels: same entry points as pretrain_src/model/bev_utils.py
 (`bevpos_polar`, `PointCloud.forward`, `PointCloud.project_bev`) plus the fused `lift_splat` used by the
 pre-training wrapper (pretrain_cmt.py:114-167)."""
 import math

@@ -1,4 +1,4 @@
-"""GlocalTextPathNavCMT on the B200 kernels -- the agents' per-step API (map_nav_src/models/vilmodel.py:705-912):
+"""GlocalTextPathNavCMT on the H100 kernels -- the agents' per-step API (map_nav_src/models/vilmodel.py:705-912):
 `forward(mode, batch)` with mode in {'language', 'panorama', 'navigation'}.  Same parameter names as the reference
 (heads live at the top level, as after `vlnbert_init.py:39-46` re-prefixing).  Tensors crossing the API are fp32
 like the reference's (the agents average / cache them on the host side); inside, activations are bf16."""

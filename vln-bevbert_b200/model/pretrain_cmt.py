@@ -1,4 +1,4 @@
-"""GlocalTextPathCMTPreTraining on the B200 kernels -- drop-in for pretrain_src/model/pretrain_cmt.py.
+"""GlocalTextPathCMTPreTraining on the H100 kernels -- drop-in for pretrain_src/model/pretrain_cmt.py.
 
 `forward(batch, task, compute_loss=True)` has the reference's contract (pretrain_cmt.py:169-238): it takes
 the collated batch dict, runs the BEV

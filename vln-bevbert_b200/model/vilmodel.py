@@ -1,8 +1,8 @@
-"""GlocalTextPathCMT on the B200 kernels -- drop-in for pretrain_src/model/vilmodel.py.
+"""GlocalTextPathCMT on the H100 kernels -- drop-in for pretrain_src/model/vilmodel.py.
 
 Same class names, constructor argument (an HF-style config), forward signatures and state_dict keys as the
 reference (SURVEY.md 8b); the nn.Linear / nn.LayerNorm / nn.Embedding / nn.MultiheadAttention children are
-parameter containers only -- all arithmetic runs in the sm_100a kernels through `blocks.run_block`.
+parameter containers only -- all arithmetic runs in the sm_90a kernels through `blocks.run_block`.
 nn.Dropout children are kept so that the reference's `set_dropout(model, p)` (utils/misc.py:19-25) still
 controls the probabilities.
 """
