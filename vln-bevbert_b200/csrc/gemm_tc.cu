@@ -1,10 +1,11 @@
 // Batched bf16 GEMM for sm_90a: TMA -> 128B-swizzled shared memory -> wgmma (fp32 accumulators in registers) ->
 // register epilogue with fused bias / GELU / ReLU / gelu' / dropout / residual.
 //
-// Persistent, warp-specialised: warps 0..7 = two consumer warpgroups (warpgroup c owns accumulator rows
-// 64 c .. 64 c + 63 of the tile, issues its wgmma and runs its own epilogue), warp 8 = TMA producer (one lane).
-// One CTA per SM; the producer runs ahead through a ring of shared-memory stages, so the next tile's operands arrive
-// while the consumers are in the epilogue of the current one.
+// Persistent, warp-specialised, ping-pong: warpgroup 0 is the TMA producer (one lane issues), warpgroups 1 and 2 are
+// consumers that each own whole output tiles and alternate over the CTA's tile sequence.  The two consumers take turns
+// in the main loop, so one warpgroup's epilogue runs while the other's MMAs keep the tensor cores busy.  setmaxnreg
+// moves registers from the producer to the consumers (a 128 x 128 fp32 accumulator is 128 registers per thread).
+// One CTA per SM; the producer runs ahead through a ring of shared-memory stages in tile order.
 //
 // Tile: 128 (M) x BN (N, 64 or 128) x 64 (K) per pipeline stage. Operands may be K-major or MN-major (transposed in
 // memory; wgmma reads either from shared memory), which gives all of  X*W^T (forward), dY*W (dX) and dY^T*X (dW)
@@ -28,7 +29,10 @@ namespace bb {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int NUM_THREADS = 288;  // 2 consumer warpgroups + 1 producer warp
+constexpr int CONSUMER_THREADS = 128;             // one warpgroup
+constexpr int NUM_THREADS = 3 * CONSUMER_THREADS;  // producer warpgroup + 2 consumer warpgroups
+constexpr int PRODUCER_REGS = 40;                  // 128 x 40 + 256 x 232 <= 64 K registers per SM
+constexpr int CONSUMER_REGS = 232;
 constexpr int MAX_STAGES = 8;
 
 struct GemmKParams {
@@ -84,70 +88,84 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmKParams& p, int tile)
 
 __device__ __forceinline__ float bf2f(__nv_bfloat16 v) { return __bfloat162float(v); }
 
-// Epilogue of two adjacent output columns (col, col + 1) of one row; col is even.  EPI selects the features at compile
-// time: 0 = every feature (activation, second output, gelu'/relu' multiply, dropout, residual add, any store),
-// 1 = plain (alpha, optional bias, bf16 or fp32 store), 2 = fp32 atomic accumulate (split-K weight gradients).
+// Epilogue variants.  GENERIC decides every feature at run time (activation, second output, gelu'/relu' multiply,
+// dropout, residual add, any store); the others fix at compile time the feature combinations the model launches, so
+// their per-element code is short and free of branches.  Dropout and bias stay run-time switches everywhere.
+enum : int {
+  EPI_GENERIC = 0,
+  EPI_PLAIN = 1,       // alpha, bias; bf16 or fp32 store
+  EPI_ATOMIC = 2,      // alpha, bias; fp32 atomic accumulate (split-K weight gradients)
+  EPI_GELU_PRE = 3,    // bf16 pre-activation to aux_out, GELU, dropout; bf16 store
+  EPI_MUL_DGELU = 4,   // * gelu'(aux_in), dropout; bf16 store
+  EPI_MUL_DRELU = 5,   // * relu'(aux_in), dropout; bf16 store
+  EPI_ADD = 6,         // dropout, + add_in; bf16 store
+  EPI_COUNT = 7
+};
+
 template <int EPI>
-__device__ __forceinline__ void epi_pair(const GemmKParams& p, long long row_off, int col, float v0, float v1,
-                                         bool add_bias) {
-  const bool two = col + 1 < p.N;
-  const bool vec = two && p.vec_ok;
+__device__ __forceinline__ int epi_mul_of(const GemmKParams& p) {
+  return EPI == EPI_GENERIC ? p.epi_mul : (EPI == EPI_MUL_DGELU ? 1 : EPI == EPI_MUL_DRELU ? 2 : 0);
+}
+template <int EPI>
+__device__ __forceinline__ bool epi_add_of(const GemmKParams& p) {
+  return EPI == EPI_GENERIC ? p.add_in != nullptr : EPI == EPI_ADD;
+}
+
+// Epilogue of two adjacent output columns (col, col + 1) of one row at element offset `off`; col is even.  b0 / b1 are
+// the bias of the two columns (added when add_bias), mul_in / add_v the aux_in and add_in values of the pair, all read
+// by the caller.  EDGE: the pair may straddle the last column or lack the alignment of a paired store.
+template <int EPI, bool EDGE>
+__device__ __forceinline__ void epi_pair(const GemmKParams& p, long long off, int col, float v0, float v1,
+                                         bool add_bias, float b0, float b1, __nv_bfloat162 mul_in,
+                                         __nv_bfloat162 add_v) {
+  const bool two = !EDGE || col + 1 < p.N;
+  const bool vec = !EDGE || (two && p.vec_ok);
+  const bool generic = EPI == EPI_GENERIC;
+  const bool aux_out = generic ? p.aux_out != nullptr : EPI == EPI_GELU_PRE;
+  const int act = generic ? p.act : (EPI == EPI_GELU_PRE ? 1 : 0);
+  const int mul = epi_mul_of<EPI>(p);
+  const bool drop = (generic || EPI >= EPI_GELU_PRE) && p.drop_thresh != 0;
+  const bool out_f32 = EPI == EPI_ATOMIC || ((generic || EPI == EPI_PLAIN) && p.out_f32 != 0);
+  const bool atomic = EPI == EPI_ATOMIC || (generic && p.atomic != 0);
+  const bool fast_gelu = generic && p.fast_gelu;
   v0 *= p.alpha;
   v1 *= p.alpha;
   if (add_bias) {
-    v0 += __ldg(p.bias + col);
-    if (two) v1 += __ldg(p.bias + col + 1);
+    v0 += b0;
+    if (two) v1 += b1;
   }
-  const long long off = row_off + col;
-  const bool out_f32 = EPI == 2 ? true : (p.out_f32 != 0);
-  const bool atomic = EPI == 2 ? true : (EPI == 1 ? false : p.atomic != 0);
-  if constexpr (EPI == 0) {
-    if (p.aux_out != nullptr) {
-      if (vec) *reinterpret_cast<__nv_bfloat162*>(p.aux_out + off) = __floats2bfloat162_rn(v0, v1);
-      else {
-        p.aux_out[off] = __float2bfloat16(v0);
-        if (two) p.aux_out[off + 1] = __float2bfloat16(v1);
-      }
+  if (aux_out) {
+    if (vec) *reinterpret_cast<__nv_bfloat162*>(p.aux_out + off) = __floats2bfloat162_rn(v0, v1);
+    else {
+      p.aux_out[off] = __float2bfloat16(v0);
+      if (two) p.aux_out[off + 1] = __float2bfloat16(v1);
     }
-    if (p.act == 1) {
-      if (p.fast_gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
-      else { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-    } else if (p.act == 2) {
-      v0 = fmaxf(v0, 0.0f);
-      v1 = fmaxf(v1, 0.0f);
+  }
+  if (act == 1) {
+    if (fast_gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+    else { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+  } else if (act == 2) {
+    v0 = fmaxf(v0, 0.0f);
+    v1 = fmaxf(v1, 0.0f);
+  }
+  if (mul != 0) {
+    const float2 a = __bfloat1622float2(mul_in);
+    if (mul == 1) {
+      if (fast_gelu) { v0 *= dgelu_fast(a.x); v1 *= dgelu_fast(a.y); }
+      else { v0 *= dgelu_erf(a.x); v1 *= dgelu_erf(a.y); }
+    } else {
+      v0 = a.x > 0.0f ? v0 : 0.0f;
+      v1 = a.y > 0.0f ? v1 : 0.0f;
     }
-    if (p.epi_mul != 0) {
-      float a0, a1 = 0.0f;
-      if (vec) {
-        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.aux_in + off));
-        a0 = a.x;
-        a1 = a.y;
-      } else {
-        a0 = bf2f(p.aux_in[off]);
-        if (two) a1 = bf2f(p.aux_in[off + 1]);
-      }
-      if (p.epi_mul == 1) {
-        if (p.fast_gelu) { v0 *= dgelu_fast(a0); v1 *= dgelu_fast(a1); }
-        else { v0 *= dgelu_erf(a0); v1 *= dgelu_erf(a1); }
-      } else {
-        v0 = a0 > 0.0f ? v0 : 0.0f;
-        v1 = a1 > 0.0f ? v1 : 0.0f;
-      }
-    }
-    if (p.drop_thresh != 0) {
-      v0 = drop_keep(p.drop_seed, (uint64_t)off, p.drop_thresh) ? v0 * p.drop_scale : 0.0f;
-      v1 = drop_keep(p.drop_seed, (uint64_t)(off + 1), p.drop_thresh) ? v1 * p.drop_scale : 0.0f;
-    }
-    if (p.add_in != nullptr) {
-      if (vec) {
-        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.add_in + off));
-        v0 += a.x;
-        v1 += a.y;
-      } else {
-        v0 += bf2f(p.add_in[off]);
-        if (two) v1 += bf2f(p.add_in[off + 1]);
-      }
-    }
+  }
+  if (drop) {
+    v0 = drop_keep(p.drop_seed, (uint64_t)off, p.drop_thresh) ? v0 * p.drop_scale : 0.0f;
+    v1 = drop_keep(p.drop_seed, (uint64_t)(off + 1), p.drop_thresh) ? v1 * p.drop_scale : 0.0f;
+  }
+  if (epi_add_of<EPI>(p)) {
+    const float2 a = __bfloat1622float2(add_v);
+    v0 += a.x;
+    if (two) v1 += a.y;
   }
   if (out_f32) {
     float* D = reinterpret_cast<float*>(p.D) + off;
@@ -174,33 +192,104 @@ __device__ __forceinline__ void epi_pair(const GemmKParams& p, long long row_off
   }
 }
 
+// The bf16 pair (off, off + 1) of an epilogue input; the second element reads as 0 when it is past the last column.
+template <bool EDGE>
+__device__ __forceinline__ __nv_bfloat162 load_pair(const __nv_bfloat16* src, long long off, bool two, bool vec) {
+  if (!EDGE || vec) return __ldg(reinterpret_cast<const __nv_bfloat162*>(src + off));
+  return __halves2bfloat162(src[off], two ? src[off + 1] : __float2bfloat16(0.0f));
+}
+
+// Epilogue of one 128 x BN tile straight from a warpgroup's accumulator registers: acc[hh] holds rows 64 hh .. 64 hh + 63
+// in the wgmma fragment order (thread rows r0, r0 + 8; columns 8 j + cq, + 1).  With only four warps per warpgroup
+// nothing hides a load's latency, so the loads of a group of JG column pairs (bias, aux_in, add_in for the thread's
+// four rows) are all issued before the group's first store.
+template <int BN, int EPI, bool EDGE>
+__device__ __forceinline__ void epilogue(const GemmKParams& p, const TileCoord& t, const float (&acc)[2][BN / 2], int r0,
+                                         int cq) {
+  constexpr int JG = 4;
+  const int n0 = t.n_tile * BN;
+  const bool add_bias = p.bias != nullptr && t.split == 0;
+  const bool mul = epi_mul_of<EPI>(p) != 0;
+  const bool add = epi_add_of<EPI>(p);
+  const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
+  long long row_off[4];
+  bool row_ok[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int row = t.m_tile * BLOCK_M + 64 * (r >> 1) + r0 + 8 * (r & 1);
+    row_ok[r] = !EDGE || row < p.M;
+    row_off[r] = batch_off + (long long)row * p.ldd;
+  }
+#pragma unroll
+  for (int j0 = 0; j0 < BN / 8; j0 += JG) {
+    float b[JG][2];
+    __nv_bfloat162 mul_in[JG][4], add_v[JG][4];
+#pragma unroll
+    for (int jj = 0; jj < JG; ++jj) {
+      const int col = n0 + 8 * (j0 + jj) + cq;
+      const bool col_ok = !EDGE || col < p.N;
+      const bool two = !EDGE || col + 1 < p.N;
+      const bool vec = !EDGE || (two && p.vec_ok);
+      b[jj][0] = add_bias && col_ok ? __ldg(p.bias + col) : 0.0f;
+      b[jj][1] = add_bias && col_ok && two ? __ldg(p.bias + col + 1) : 0.0f;
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const bool ok = col_ok && row_ok[r];
+        mul_in[jj][r] = mul && ok ? load_pair<EDGE>(p.aux_in, row_off[r] + col, two, vec) : __nv_bfloat162();
+        add_v[jj][r] = add && ok ? load_pair<EDGE>(p.add_in, row_off[r] + col, two, vec) : __nv_bfloat162();
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < JG; ++jj) {
+      const int j = j0 + jj;
+      const int col = n0 + 8 * j + cq;
+      if (EDGE && col >= p.N) continue;
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int hh = r >> 1, h = r & 1;
+        if (row_ok[r])
+          epi_pair<EPI, EDGE>(p, row_off[r] + col, col, acc[hh][4 * j + 2 * h], acc[hh][4 * j + 2 * h + 1], add_bias,
+                              b[jj][0], b[jj][1], mul_in[jj][r], add_v[jj][r]);
+      }
+    }
+  }
+}
+
 template <int BN, int TA, int TB>
 __device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
   if constexpr (BN == 64) wgmma_m64n64_ss<TA, TB>(acc, da, db, scale_d);
   else wgmma_m64n128_ss<TA, TB>(acc, da, db, scale_d);
 }
 
-// k-blocks [kb0, kb1) of one tile into this warpgroup's accumulators.  TA / TB (operand MN-major) are template
-// parameters so that the whole loop is free of branches around the asynchronous MMAs.
+// k-blocks [kb0, kb1) of one 128 x BN tile into this warpgroup's accumulators (two m64 wgmma per k16 step; both read
+// the same B tile).  TA / TB (operand MN-major) are template parameters so that the whole loop is free of branches
+// around the asynchronous MMAs.  Once the last MMAs are issued, the other consumer warpgroup is let into its main loop
+// (ordered barrier `next_bar`, when it has a next tile); then the MMAs are drained and the last stage is released.
 template <int BN, int TA, int TB>
-__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint8_t* smem, int stage_bytes, uint64_t* full_bar,
-                                         uint64_t* empty_bar, int stages, int& stage, uint32_t& phase, int kb0, int kb1,
-                                         int wg, int lane) {
+__device__ __forceinline__ void mainloop(float (&acc)[2][BN / 2], uint8_t* smem, int stage_bytes, uint64_t* full_bar,
+                                         uint64_t* empty_bar, int stages, int stage, uint32_t phase, int kb0, int kb1,
+                                         int lane, int next_bar) {
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_u32(smem + stage * stage_bytes) + wg * 8192;
-    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + A_STAGE_BYTES;
-    fence_regs(acc);
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+    const uint32_t sb = sa + A_STAGE_BYTES;
+    fence_regs(acc[0]);
+    fence_regs(acc[1]);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < BLOCK_K / 16; ++k) {
-      const uint64_t da = TA ? wgmma_desc(sa + k * 2048, 8192, 1024) : wgmma_desc(sa + k * 32, 16, 1024);
       const uint64_t db = TB ? wgmma_desc(sb + k * 2048, 8192, 1024) : wgmma_desc(sb + k * 32, 16, 1024);
-      wgmma_tile<BN, TA, TB>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const uint32_t s = sa + hh * 8192;
+        const uint64_t da = TA ? wgmma_desc(s + k * 2048, 8192, 1024) : wgmma_desc(s + k * 32, 16, 1024);
+        wgmma_tile<BN, TA, TB>(acc[hh], da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+      }
     }
     wgmma_commit();
-    fence_regs(acc);
+    fence_regs(acc[0]);
+    fence_regs(acc[1]);
     // at most the group just issued is in flight: the previous stage has been read and can be refilled
     wgmma_wait<1>();
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -210,8 +299,10 @@ __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint8_t* smem, in
       phase ^= 1;
     }
   }
+  if (next_bar >= 0) named_bar_arrive(next_bar, 2 * CONSUMER_THREADS);
   wgmma_wait<0>();
-  fence_regs(acc);
+  fence_regs(acc[0]);
+  fence_regs(acc[1]);
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 }
 
@@ -227,15 +318,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
 
+  const int wg = threadIdx.x / CONSUMER_THREADS;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);   // lane 0 of every consumer warp
+      mbar_init(&empty_bar[i], 4);   // lane 0 of each warp of the consumer warpgroup that read the stage
     }
     fence_mbar_init();
   }
@@ -246,9 +338,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   pdl_trigger();
   if (p.prof && threadIdx.x == 0) atomicMin(p.prof, (unsigned long long)gtimer());
 
-  if (warp == 8) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer (one lane), stages in tile order
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -284,47 +377,46 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
     }
   } else {
-    // ------------------------------------------------------------------ consumers: wgmma mainloop + epilogue
-    const int wg = warp >> 2;                       // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
-    const int r0 = (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8 of the warpgroup's 64
+    // ------------------------------------------------------------------ consumers: ping-pong over the CTA's tiles
+    // Consumer warpgroup c owns the CTA's local tiles lt = c, c + 2, ...  Main loops take turns through two named
+    // barriers: before the main loop of tile lt > 0 a warpgroup waits on its own barrier (1 + c) for the other one to
+    // have issued all MMAs of tile lt - 1, so each epilogue runs under the other warpgroup's MMAs.  A warpgroup signals
+    // only when the other one has a next tile, so no arrival is left pending when the kernel ends.
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int c = wg - 1;
+    const int r0 = (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8 of each 64-row half
     const int cq = 2 * (lane & 3);                  // fragment column offset within each 8-column group
-    int stage = 0;
-    uint32_t phase = 0;
+    uint32_t kdone = 0;   // k-blocks the producer queued for the CTA's earlier tiles: position in the stage ring
     int lt = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
       const TileCoord t = decode_tile(p, tile);
       const int kb0 = t.split * p.kb_per_split;
       const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-      const bool stamp = p.trace && lt < 16 && threadIdx.x == 0;
+      const uint32_t kpos = kdone;
+      kdone += kb1 - kb0;
+      if ((lt & 1) != c) continue;
+      const int stage = (int)(kpos % (uint32_t)p.stages);
+      const uint32_t phase = (kpos / (uint32_t)p.stages) & 1;
+      const int next_bar = tile + (int)gridDim.x < total_tiles ? 2 - c : -1;
+      if (lt > 0) named_bar_sync(1 + c, 2 * CONSUMER_THREADS);
+      const bool stamp = p.trace && lt < 16 && (threadIdx.x % CONSUMER_THREADS) == 0;
       if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 0] = gtimer();
-      float acc[BN / 2];
+      float acc[2][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.0f;
       switch (p.a_mn * 2 + p.b_mn) {
-        case 0: mainloop<BN, 0, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
-        case 1: mainloop<BN, 0, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
-        case 2: mainloop<BN, 1, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
-        default: mainloop<BN, 1, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, wg, lane); break;
+        case 0: mainloop<BN, 0, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, lane, next_bar); break;
+        case 1: mainloop<BN, 0, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, lane, next_bar); break;
+        case 2: mainloop<BN, 1, 0>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, lane, next_bar); break;
+        default: mainloop<BN, 1, 1>(acc, smem, STAGE_BYTES, full_bar, empty_bar, p.stages, stage, phase, kb0, kb1, lane, next_bar); break;
       }
       if (stamp) {
         p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 1] = gtimer();
         p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 2] = gtimer();
       }
-      // ---- epilogue straight from the accumulator registers
-      const int n0 = t.n_tile * BN;
-      const bool add_bias = p.bias != nullptr && t.split == 0;
-      const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = t.m_tile * BLOCK_M + wg * 64 + r0 + 8 * h;
-        if (row >= p.M) continue;
-        const long long row_off = batch_off + (long long)row * p.ldd;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int col = n0 + 8 * j + cq;
-          if (col < p.N) epi_pair<EPI>(p, row_off, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], add_bias);
-        }
-      }
+      const bool interior = p.vec_ok && (t.m_tile + 1) * BLOCK_M <= p.M && (t.n_tile + 1) * BN <= p.N;
+      if (interior) epilogue<BN, EPI, false>(p, t, acc, r0, cq);
+      else epilogue<BN, EPI, true>(p, t, acc, r0, cq);
       if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 3] = gtimer();
     }
   }
@@ -431,6 +523,21 @@ static unsigned long long* g_prof_buf = nullptr;
 static size_t g_prof_cap = 0;
 
 static long long* g_trace = nullptr;   // bb_gemm_trace(): device buffer of (grid x 16 x 4) timestamps, debug only
+
+typedef void (*GemmKernel)(CUtensorMap, CUtensorMap, GemmKParams, int);
+template <int BN>
+static GemmKernel gemm_kernel(int epi) {
+  switch (epi) {
+    case EPI_PLAIN: return gemm_tc_kernel<BN, EPI_PLAIN>;
+    case EPI_ATOMIC: return gemm_tc_kernel<BN, EPI_ATOMIC>;
+    case EPI_GELU_PRE: return gemm_tc_kernel<BN, EPI_GELU_PRE>;
+    case EPI_MUL_DGELU: return gemm_tc_kernel<BN, EPI_MUL_DGELU>;
+    case EPI_MUL_DRELU: return gemm_tc_kernel<BN, EPI_MUL_DRELU>;
+    case EPI_ADD: return gemm_tc_kernel<BN, EPI_ADD>;
+    default: return gemm_tc_kernel<BN, EPI_GENERIC>;
+  }
+}
+
 static int g_num_sms = 0;
 static int g_smem_optin = 0;
 static int init_device_info() {
@@ -443,8 +550,10 @@ static int init_device_info() {
   auto set = [&](auto kernel) {
     ok = ok && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin) == cudaSuccess;
   };
-  set(gemm_tc_kernel<64, 0>); set(gemm_tc_kernel<64, 1>); set(gemm_tc_kernel<64, 2>);
-  set(gemm_tc_kernel<128, 0>); set(gemm_tc_kernel<128, 1>); set(gemm_tc_kernel<128, 2>);
+  for (int epi = 0; epi < EPI_COUNT; ++epi) {
+    set(gemm_kernel<64>(epi));
+    set(gemm_kernel<128>(epi));
+  }
   if (!ok) return set_error("cudaFuncSetAttribute(max dynamic smem) failed for gemm_tc_kernel");
   return 0;
 }
@@ -538,14 +647,18 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
     p.vec_ok = ok ? 1 : 0;
   }
 
-  // epilogue variant (BB_GEMM_EPI=0 forces the generic one, for A/B runs)
-  static const int epi_mode = [] {
-    const char* e_ = getenv("BB_GEMM_EPI");
-    return (e_ && e_[0] == '0') ? 0 : 1;
-  }();
-  int epi = 0;
-  const bool featureless = !p.act && !p.aux_out && !p.epi_mul && !p.add_in && !p.drop_thresh;
-  if (epi_mode && featureless) epi = p.atomic ? (p.bias ? 0 : 2) : 1;
+  // epilogue variant: the compile-time one for the feature combination, else the generic one (which also carries the
+  // BB_FAST_GELU experiment)
+  int epi = EPI_GENERIC;
+  const bool plain = !p.act && !p.aux_out && !p.epi_mul && !p.add_in && !p.drop_thresh;
+  if (plain) {
+    epi = p.atomic ? EPI_ATOMIC : EPI_PLAIN;
+  } else if (!p.out_f32 && !p.fast_gelu) {
+    if (p.act == 1 && p.aux_out && !p.epi_mul && !p.add_in) epi = EPI_GELU_PRE;
+    else if (!p.act && !p.aux_out && p.epi_mul == 1 && !p.add_in) epi = EPI_MUL_DGELU;
+    else if (!p.act && !p.aux_out && p.epi_mul == 2 && !p.add_in) epi = EPI_MUL_DRELU;
+    else if (!p.act && !p.aux_out && !p.epi_mul && p.add_in) epi = EPI_ADD;
+  }
 
   const int stage_bytes = A_STAGE_BYTES + bn * BLOCK_K * 2;
   int stages = (g_smem_optin - 1024 - 256) / stage_bytes;
@@ -582,16 +695,8 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
     p.prof = g_prof_buf + 2 * g_prof_used;
     ++g_prof_used;
   }
-  auto go = [&](auto kernel) { bb::launch_pdl(kernel, grid, NUM_THREADS, smem_bytes, stream, ta, tb, p, (int)total); };
-  if (bn == 64) {
-    if (epi == 1) go(gemm_tc_kernel<64, 1>);
-    else if (epi == 2) go(gemm_tc_kernel<64, 2>);
-    else go(gemm_tc_kernel<64, 0>);
-  } else {
-    if (epi == 1) go(gemm_tc_kernel<128, 1>);
-    else if (epi == 2) go(gemm_tc_kernel<128, 2>);
-    else go(gemm_tc_kernel<128, 0>);
-  }
+  GemmKernel kernel = bn == 64 ? gemm_kernel<64>(epi) : gemm_kernel<128>(epi);
+  bb::launch_pdl(kernel, grid, NUM_THREADS, smem_bytes, stream, ta, tb, p, (int)total);
   count_launch();
   return check_launch("gemm_tc_kernel");
 }

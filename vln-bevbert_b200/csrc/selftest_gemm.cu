@@ -257,6 +257,15 @@ int main(int argc, char** argv) {
       {"perf_attn_s441", 441, 441, 64, 12, 32, 0, 0, 2304, 64, 441LL * 2304, 2304, 64, 441LL * 2304, 448, 441LL * 448,
        12LL * 441 * 448, 1, 1, 0, 0, 0, 0, 0, 0, 0.125f, 20},
       {"perf_dw", 768, 3072, 14112, 1, 1, 1, 1, 768, 0, 0, 3072, 0, 0, 3072, 0, 0, 1, 8, 0, 0, 0, 0, 0, 0, 1.f, 20},
+      // FFN up-projection backward dX: (dY W2) * gelu'(pre)
+      {"perf_dgelu", 14112, 3072, 768, 1, 1, 0, 1, 768, 0, 0, 3072, 0, 0, 3072, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 1.f, 20},
+      // QKV backward dX with the residual gradient added
+      {"perf_qkv_dx", 14112, 768, 2304, 1, 1, 0, 1, 2304, 0, 0, 768, 0, 0, 768, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 1.f, 20},
+      // ping-pong tile schedules (tile counts for a 132-SM H100): 3 tiles per CTA, so the first consumer warpgroup
+      // takes one tile more than the second; a single tile; one tile more than the grid (one CTA runs two)
+      {"pp_odd_tiles", 4224, 1536, 256, 1, 1, 0, 0, 256, 0, 0, 256, 0, 0, 1536, 0, 0, 0, 1, 1, 1, 1, 0, 0, 0, 1.f, 0},
+      {"pp_one_tile", 100, 60, 512, 1, 1, 0, 0, 512, 0, 0, 512, 0, 0, 60, 0, 0, 0, 1, 0, 1, 0, 0, 1, 0, 1.f, 0},
+      {"pp_grid_plus_1", 17024, 128, 192, 1, 1, 0, 1, 192, 0, 0, 128, 0, 0, 128, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 1.f, 0},
   };
   if (argc < 2 || !strcmp(argv[1], "list")) {
     for (auto& c : cases) printf("%s\n", c.name);
