@@ -31,6 +31,23 @@ void bb_reset_launch_count(void);
  * value, so masks are still replayed exactly).  Synchronous (cudaMemcpyToSymbol); call it once, outside capture. */
 int bb_set_drop_salt_ptr(const uint64_t* device_word);
 
+/* Deterministic mode.  on = 1: every kernel gives bit-identical results for bit-identical inputs on the same build and
+ * GPU model, whatever the scheduling (side stream, CUDA-graph replay, concurrent work).  Reductions across CTAs (split-K
+ * weight gradients, LayerNorm dgamma / dbeta, bias column sums, graph-bias gradients, the gradient sum of squares)
+ * store partials to the workspace and add them in a fixed order; no CTA waits on another.  The atomic scatter-adds
+ * (bb_embed_scatter_grad's word table, bb_scatter_add_rows, bb_segment_wsum_bwd) fail in this mode: their callers sort
+ * by destination and use bb_scatter_rows_sorted.  A launch without a deterministic implementation (the fused-scores
+ * graph-bias gradient of bb_attn_scores) fails.  on = 2: the same, except that such a launch runs (the caller warns).
+ * on = 0 (default): fp32 atomics, as before.  Host state, takes effect at the next launch. */
+int bb_set_deterministic(int on);
+/* Workspaces of the deterministic mode, owned by the caller, 256-byte aligned, `bytes` each, zero-filled before
+ * registration: the first 64 KB hold split-K arrival counters that every launch leaves at zero.  Launches on the
+ * registered side stream (bb_set_side_stream) use side_ws, every other launch main_ws.  A deterministic launch whose
+ * workspace is missing or too small fails and bb_last_error() gives the size it needs: 64 KB plus, for a split-K GEMM,
+ * split x output tiles x 128 x tile width x 4 bytes (tiles 64 or 128 wide), for the other reductions a few MB at most.
+ * NULL, NULL, 0 unregisters. */
+int bb_set_det_workspace(void* main_ws, void* side_ws, int64_t bytes);
+
 /* ---------------------------------------------------------------------------------------------
  * Batched bf16 GEMM on wgmma tensor cores, TMA-fed, fp32 accumulation in registers.
  *   D[b] = epi( alpha * A[b] (M x K) * B[b]^T (N x K) )
@@ -183,6 +200,15 @@ int bb_embed_scatter_grad(const int64_t* ids, const float* dz, int64_t ntok, int
  * out[idx[r], :] += in[r, :] in f32. */
 int bb_gather_rows_bf16(const void* in, const int64_t* idx, int64_t nout, int H, void* out, void* stream);
 int bb_scatter_add_rows(const void* in_bf16, const int64_t* idx, int64_t nin, int H, float* out_f32, void* stream);
+/* Deterministic scatter-add by destination.  dst_sorted (n,) is sorted ascending and stable, so entries with the same
+ * destination keep ascending source order; for each run of entries e1 < e2 < ... with dst_sorted == d >= 0:
+ *   out_f32[d, :] += ((t_e1 + t_e2) + ...),   t_e = w[e] * src[src_row[e], :]  (one rounded fp32 product, no FMA),
+ * or t_e = src[src_row[e], :] when w is NULL; entries with dst_sorted < 0 are dropped.  src is f32 (src_f32 = 1) or
+ * the activation type, rows of width H (a multiple of 8); src and out 16-byte aligned.  With a stable sort of the
+ * destinations, this is the deterministic form of bb_scatter_add_rows, bb_segment_wsum_bwd and the word-table gradient
+ * of bb_embed_scatter_grad. */
+int bb_scatter_rows_sorted(const void* src, int src_f32, const int64_t* src_row, const float* w,
+                           const int64_t* dst_sorted, int64_t n, int H, float* out_f32, void* stream);
 
 /* bf16 -> bf16 inverted dropout with the same counter-based RNG as everywhere else (element index = counter):
  * regenerates a forward mask in backward.  src may equal dst. */

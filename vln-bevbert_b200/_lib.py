@@ -97,6 +97,8 @@ _SIGNATURES = {
     "bb_reset_launch_count": (None, []),
     "bb_gemm_bf16": (c_int, [C.POINTER(GemmArgs), c_void_p]),
     "bb_set_drop_salt_ptr": (c_int, [c_void_p]),
+    "bb_set_deterministic": (c_int, [c_int]),
+    "bb_set_det_workspace": (c_int, [c_void_p, c_void_p, c_i64]),
     "bb_set_act_f32": (c_int, [c_int]),
     "bb_get_act_f32": (c_int, []),
     "bb_gemm_trace": (c_int, [c_void_p]),
@@ -129,6 +131,7 @@ _SIGNATURES = {
                                       c_void_p]),
     "bb_gather_rows_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_scatter_add_rows": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
+    "bb_scatter_rows_sorted": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_dropout_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_u64, c_u32, c_float, c_void_p]),
     "bb_act_bwd_bf16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p]),
     "bb_add_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),

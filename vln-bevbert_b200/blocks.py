@@ -1034,7 +1034,10 @@ class MLMLossImpl:
         K.scale_rows_(dlog, g, m, ld)
         dE = zeros_f32(g.device, V, Hd)
         kb = (m + 63) // 64
-        K.gemm(dlog, tn, dE, V, Hd, m, lda=ld, ldb=Hd, ldd=Hd, a_mn=True, b_mn=True, split_k=1 if kb < 8 else 2)
+        # a split adds nothing to the occupancy of this many vocabulary tiles; in deterministic mode its partial tiles
+        # would need a workspace the size of dE, so the product runs unsplit there
+        split = 1 if kb < 8 or torch.are_deterministic_algorithms_enabled() else 2
+        K.gemm(dlog, tn, dE, V, Hd, m, lda=ld, ldb=Hd, ldd=Hd, a_mn=True, b_mn=True, split_k=split)
         dvb = zeros_f32(g.device, ld)
         K.colsum(dlog, ld, out=dvb)
         dtn = _empty((m, Hd), tn)

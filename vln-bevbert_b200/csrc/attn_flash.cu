@@ -49,6 +49,7 @@ struct Params {
   const float* kmask;
   const float* bias;
   float* dbias;
+  int64_t dbias_hs;   // deterministic mode: per-head partials dbias + h * dbias_hs, plain stores; 0: fp32 atomics
   int B, H, nq, nk;
   float alpha;
   uint64_t seed;
@@ -431,17 +432,23 @@ __global__ void __launch_bounds__(NT, 3) flash_bwd_dq_kernel(const Params p) {
       s[nb][2] = ex2(s[nb][2] - lse1) * (g10 - d1);
       s[nb][3] = ex2(s[nb][3] - lse1) * (g11 - d1);
     }
-    if (p.dbias) {   // graph-bias gradient (global map encoder): sum over heads with fp32 atomics
-      float* db0 = r0 < p.nq ? p.dbias + ((int64_t)b * p.nq + r0) * p.nk : nullptr;
-      float* db1 = r0 + 8 < p.nq ? p.dbias + ((int64_t)b * p.nq + r0 + 8) * p.nk : nullptr;
+    if (p.dbias) {   // graph-bias gradient (global map encoder): sum over heads with fp32 atomics or per-head partials
+      float* dbh = p.dbias + h * p.dbias_hs;
+      float* db0 = r0 < p.nq ? dbh + ((int64_t)b * p.nq + r0) * p.nk : nullptr;
+      float* db1 = r0 + 8 < p.nq ? dbh + ((int64_t)b * p.nq + r0 + 8) * p.nk : nullptr;
 #pragma unroll
       for (int nb = 0; nb < 8; ++nb) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = j * BN + nb * 8 + 2 * t + e;
           if (col < p.nk) {
-            if (db0) atomicAdd(db0 + col, s[nb][e]);
-            if (db1) atomicAdd(db1 + col, s[nb][2 + e]);
+            if (p.dbias_hs) {
+              if (db0) db0[col] = s[nb][e];
+              if (db1) db1[col] = s[nb][2 + e];
+            } else {
+              if (db0) atomicAdd(db0 + col, s[nb][e]);
+              if (db1) atomicAdd(db1 + col, s[nb][2 + e]);
+            }
           }
         }
       }
@@ -619,10 +626,16 @@ extern "C" int bb_flash_bwd(const bb_flash_args* a, void* stream) {
   if (fat::bwd_supported(a)) return fat::launch_bwd(a, stream);   // wgmma / TMA core (attn_tc.cu)
   const dim3 gq((unsigned)((a->nq + fa::BM - 1) / fa::BM), (unsigned)a->H, (unsigned)a->B);
   const dim3 gk((unsigned)((a->nk + fa::BM - 1) / fa::BM), (unsigned)a->H, (unsigned)a->B);
+  if (p.dbias && det_on()) {   // per-head partials, then a sum over heads in head order
+    p.dbias_hs = (int64_t)a->B * a->nq * a->nk;
+    p.dbias = det_partials((cudaStream_t)stream, (size_t)a->H * p.dbias_hs * sizeof(float), "bb_flash_bwd (graph-bias gradient)");
+    if (!p.dbias) return -1;
+  }
   launch_pdl(fa::flash_bwd_dq_kernel, gq, dim3(fa::NT), 0, (cudaStream_t)stream, p);
   launch_pdl(fa::flash_bwd_dkv_kernel, gk, dim3(fa::NT), 0, (cudaStream_t)stream, p);
   count_launch(2);
-  return check_launch("flash_bwd kernels");
+  if (int e = check_launch("flash_bwd kernels")) return e;
+  return p.dbias_hs ? det_reduce(p.dbias, a->H, p.dbias_hs, 1, a->dbias, nullptr, nullptr, (cudaStream_t)stream) : 0;
 }
 
 namespace bb { int set_salt_attn_flash(const unsigned long long* p) { return set_drop_salt_ptr_tu(p) == cudaSuccess ? 0 : -1; } }

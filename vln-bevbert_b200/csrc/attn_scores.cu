@@ -320,6 +320,9 @@ extern "C" int bb_attn_scores(const bb_attn_scores_args* a, void* stream_) {
   if (a->ldp % 8 != 0 || a->ldp < a->nk) return set_error("bb_attn_scores: ldp must be a multiple of 8 and >= nk");
   if (a->mode == 0 && !a->P) return set_error("bb_attn_scores: mode 0 needs P");
   if (a->mode == 1 && (!a->Pin || !a->dS)) return set_error("bb_attn_scores: mode 1 needs Pin and dS");
+  if (a->mode == 1 && a->dbias && det_mode() == 1)
+    return set_error("bb_attn_scores: the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient adds with fp32 atomics "
+                     "and has no deterministic implementation");
   static int num_sms = 0;
   if (!num_sms) {
     int dev = 0, optin = 0;

@@ -33,6 +33,47 @@ bool pdl_enabled() {
 }
 }  // namespace bb
 
+namespace bb {
+static int g_det = 0;
+static char* g_det_ws[2] = {nullptr, nullptr};   // main, side
+static int64_t g_det_bytes = 0;
+
+int det_mode() { return g_det; }
+
+static char* det_ws(cudaStream_t stream) { return g_det_ws[stream && stream == side_stream() ? 1 : 0]; }
+
+float* det_partials(cudaStream_t stream, size_t bytes, const char* who) {
+  char* ws = det_ws(stream);
+  const size_t need = DET_COUNTER_BYTES + bytes;
+  if (!ws || (size_t)g_det_bytes < need) {
+    char buf[300];
+    snprintf(buf, sizeof(buf),
+             "%s: deterministic mode needs a workspace of at least %zu bytes on this stream (registered: %lld); "
+             "see bb_set_det_workspace", who, need, ws ? (long long)g_det_bytes : 0LL);
+    set_error(buf);
+    return nullptr;
+  }
+  return reinterpret_cast<float*>(ws + DET_COUNTER_BYTES);
+}
+unsigned* det_counters(cudaStream_t stream) { return reinterpret_cast<unsigned*>(det_ws(stream)); }
+}  // namespace bb
+
+extern "C" int bb_set_deterministic(int on) {
+  if (on < 0 || on > 2) return bb::set_error("bb_set_deterministic: mode must be 0, 1 or 2");
+  bb::g_det = on;
+  return 0;
+}
+extern "C" int bb_set_det_workspace(void* main_ws, void* side_ws, int64_t bytes) {
+  if ((main_ws || side_ws) && bytes < (int64_t)bb::DET_COUNTER_BYTES)
+    return bb::set_error("bb_set_det_workspace: a workspace must hold at least the 64 KB of split-K counters");
+  if ((reinterpret_cast<uintptr_t>(main_ws) | reinterpret_cast<uintptr_t>(side_ws)) & 255)
+    return bb::set_error("bb_set_det_workspace: workspaces must be 256-byte aligned");
+  bb::g_det_ws[0] = static_cast<char*>(main_ws);
+  bb::g_det_ws[1] = static_cast<char*>(side_ws);
+  bb::g_det_bytes = (main_ws || side_ws) ? bytes : 0;
+  return 0;
+}
+
 extern "C" const char* bb_last_error(void) { return bb::g_err; }
 extern "C" int bb_abi_version(void) { return 1; }
 extern "C" int64_t bb_launch_count(void) { return bb::g_launches.load(); }

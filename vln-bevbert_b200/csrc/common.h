@@ -14,6 +14,22 @@ bool pdl_enabled();                      // BB_PDL env (default on)
 int make_tmap_bf16_4d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t rows, uint64_t nb1, uint64_t nb2,
                       int64_t ld, int64_t s1, int64_t s2, uint32_t box_rows);
 
+// Deterministic mode (bb_set_deterministic): every reduction across CTAs adds in a fixed order instead of with fp32
+// atomics.  Contributors store partials to a workspace with plain stores; the last-arriving CTA or a following kernel
+// sums them in order.  No CTA ever waits on another.
+int det_mode();                               // 0 off, 1 on, 2 on but paths without a deterministic kernel still run
+inline bool det_on() { return det_mode() != 0; }
+constexpr size_t DET_COUNTER_BYTES = 65536;   // split-K tile arrival counters at the start of each workspace
+cudaStream_t side_stream();                   // layers.cu: the registered side stream (bb_set_side_stream) or null
+// The workspace of a launch on `stream` (the side-stream buffer for the registered side stream, else the main one):
+// its partial-sum area after the counters, or null with the error set when it is missing or smaller than `bytes`.
+float* det_partials(cudaStream_t stream, size_t bytes, const char* who);
+unsigned* det_counters(cudaStream_t stream);  // the zeroed counters of the same workspace
+// o_k[i] += part[0][k][i] + part[1][k][i] + ... + part[nparts-1][k][i] (left to right) for k < nout, i < n; null
+// outputs are skipped.  part[p][k][i] lives at part + (p * nout + k) * n + i (rowops.cu).
+int det_reduce(const float* part, int nparts, long long n, int nout, float* o0, float* o1, float* o2,
+               cudaStream_t stream);
+
 // Launch with programmatic dependent launch allowed: the kernel may become resident while the previous kernel on
 // the stream drains; every kernel launched this way executes griddepcontrol.wait (bb::pdl_wait) before it touches
 // global memory, so ordering is unchanged and only launch latency / prologue overlap the predecessor's tail.

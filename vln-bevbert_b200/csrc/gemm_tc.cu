@@ -58,6 +58,8 @@ struct GemmKParams {
   unsigned int drop_thresh;
   float drop_scale;
   int fast_gelu;      // experiment: Abramowitz-Stegun erf on approximate MUFU ops instead of erff()
+  float* det_part;     // EPI_SPLIT_DET: fp32 partial tiles, [split][tile][128 x BN]
+  unsigned* det_cnt;   // EPI_SPLIT_DET: per-tile arrival counters (zero between launches)
   long long* trace;   // debug: per CTA and local tile 4 globaltimer stamps (mma start/end, epilogue start/end) or null
   unsigned long long* prof;   // measurement: [0] = min over CTAs of the start stamp, [1] = max of the end stamp, or null
 };
@@ -99,7 +101,8 @@ enum : int {
   EPI_MUL_DGELU = 4,   // * gelu'(aux_in), dropout; bf16 store
   EPI_MUL_DRELU = 5,   // * relu'(aux_in), dropout; bf16 store
   EPI_ADD = 6,         // dropout, + add_in; bf16 store
-  EPI_COUNT = 7
+  EPI_SPLIT_DET = 7,   // alpha, bias; split-K partials summed in split order by the last split (deterministic mode)
+  EPI_COUNT = 8
 };
 
 template <int EPI>
@@ -253,6 +256,74 @@ __device__ __forceinline__ void epilogue(const GemmKParams& p, const TileCoord& 
       }
     }
   }
+}
+
+// Deterministic split-K epilogue of one 128 x BN tile.  Every split stores alpha * acc (+ bias in split 0) to its own
+// fp32 partial tile with plain stores; then one thread of the warpgroup takes a ticket from the tile's arrival
+// counter, after a fence.  The warpgroup that arrives last adds the S partials in split order 0 .. S-1 to D and resets
+// the counter, so the counters are zero again for the next launch or graph replay.  Nobody waits for anybody.
+template <int BN, bool EDGE>
+__device__ __forceinline__ void epilogue_split_det(const GemmKParams& p, const TileCoord& t, const float (&acc)[2][BN / 2],
+                                                   int r0, int cq, int c, int* ticket) {
+  const int n0 = t.n_tile * BN;
+  const long long tile = (((long long)t.b2 * p.nb1 + t.b1) * p.m_tiles + t.m_tile) * p.n_tiles + t.n_tile;
+  const long long tiles = (long long)p.m_tiles * p.n_tiles * p.nb1 * p.nb2;
+  constexpr int TILE = BLOCK_M * BN;
+  float* mine = p.det_part + ((long long)t.split * tiles + tile) * TILE;
+  const bool add_bias = p.bias != nullptr && t.split == 0;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + cq;
+    const float b0 = add_bias && (!EDGE || col < p.N) ? __ldg(p.bias + col) : 0.0f;
+    const float b1 = add_bias && (!EDGE || col + 1 < p.N) ? __ldg(p.bias + col + 1) : 0.0f;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int hh = r >> 1, h = r & 1;
+      const int rl = 64 * hh + r0 + 8 * h;
+      float v0 = acc[hh][4 * j + 2 * h] * p.alpha, v1 = acc[hh][4 * j + 2 * h + 1] * p.alpha;
+      if (add_bias) {
+        v0 += b0;
+        v1 += b1;
+      }
+      __stcg(reinterpret_cast<float2*>(mine + rl * BN + 8 * j + cq), make_float2(v0, v1));
+    }
+  }
+  const int tid = threadIdx.x % CONSUMER_THREADS;
+  __threadfence();
+  named_bar_sync(3 + c, CONSUMER_THREADS);
+  if (tid == 0) *ticket = (int)atomicAdd(p.det_cnt + tile, 1u);
+  named_bar_sync(3 + c, CONSUMER_THREADS);
+  if (*ticket != p.split_k - 1) return;
+  __threadfence();
+  const float* first = p.det_part + tile * TILE;
+  const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
+#pragma unroll 1
+  for (int r = 0; r < 4; ++r) {
+    const int rl = 64 * (r >> 1) + r0 + 8 * (r & 1);
+    const int row = t.m_tile * BLOCK_M + rl;
+    if (EDGE && row >= p.M) continue;
+    float* drow = reinterpret_cast<float*>(p.D) + batch_off + (long long)row * p.ldd;
+#pragma unroll 4
+    for (int j = 0; j < BN / 8; ++j) {
+      const int cl = 8 * j + cq, col = n0 + cl;
+      if (EDGE && col >= p.N) continue;
+      float2 s = __ldcg(reinterpret_cast<const float2*>(first + rl * BN + cl));
+      for (int k = 1; k < p.split_k; ++k) {
+        const float2 v = __ldcg(reinterpret_cast<const float2*>(first + (long long)k * tiles * TILE + rl * BN + cl));
+        s.x += v.x;
+        s.y += v.y;
+      }
+      if (!EDGE || (col + 1 < p.N && p.vec_ok)) {
+        float2* d = reinterpret_cast<float2*>(drow + col);
+        const float2 o = *d;
+        *d = make_float2(o.x + s.x, o.y + s.y);
+      } else {
+        drow[col] += s.x;
+        if (col + 1 < p.N) drow[col + 1] += s.y;
+      }
+    }
+  }
+  if (tid == 0) p.det_cnt[tile] = 0u;
 }
 
 template <int BN, int TA, int TB>
@@ -415,8 +486,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 2] = gtimer();
       }
       const bool interior = p.vec_ok && (t.m_tile + 1) * BLOCK_M <= p.M && (t.n_tile + 1) * BN <= p.N;
-      if (interior) epilogue<BN, EPI, false>(p, t, acc, r0, cq);
-      else epilogue<BN, EPI, true>(p, t, acc, r0, cq);
+      if constexpr (EPI == EPI_SPLIT_DET) {
+        int* ticket = reinterpret_cast<int*>(empty_bar + MAX_STAGES) + c;
+        if (interior) epilogue_split_det<BN, false>(p, t, acc, r0, cq, c, ticket);
+        else epilogue_split_det<BN, true>(p, t, acc, r0, cq, c, ticket);
+      } else {
+        if (interior) epilogue<BN, EPI, false>(p, t, acc, r0, cq);
+        else epilogue<BN, EPI, true>(p, t, acc, r0, cq);
+      }
       if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 3] = gtimer();
     }
   }
@@ -534,6 +611,7 @@ static GemmKernel gemm_kernel(int epi) {
     case EPI_MUL_DGELU: return gemm_tc_kernel<BN, EPI_MUL_DGELU>;
     case EPI_MUL_DRELU: return gemm_tc_kernel<BN, EPI_MUL_DRELU>;
     case EPI_ADD: return gemm_tc_kernel<BN, EPI_ADD>;
+    case EPI_SPLIT_DET: return gemm_tc_kernel<BN, EPI_SPLIT_DET>;
     default: return gemm_tc_kernel<BN, EPI_GENERIC>;
   }
 }
@@ -652,7 +730,8 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   int epi = EPI_GENERIC;
   const bool plain = !p.act && !p.aux_out && !p.epi_mul && !p.add_in && !p.drop_thresh;
   if (plain) {
-    epi = p.atomic ? EPI_ATOMIC : EPI_PLAIN;
+    // accumulate without a split has one writer per element, so its atomic add is already deterministic
+    epi = p.atomic ? (det_on() && p.split_k > 1 ? EPI_SPLIT_DET : EPI_ATOMIC) : EPI_PLAIN;
   } else if (!p.out_f32 && !p.fast_gelu) {
     if (p.act == 1 && p.aux_out && !p.epi_mul && !p.add_in) epi = EPI_GELU_PRE;
     else if (!p.act && !p.aux_out && p.epi_mul == 1 && !p.add_in) epi = EPI_MUL_DGELU;
@@ -687,6 +766,13 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   const long long total = (long long)p.m_tiles * p.n_tiles * nb1 * nb2 * p.split_k;
   if (total > 0x7fffffffLL) return set_error("bb_gemm_bf16: too many tiles");
   const int grid = total < g_num_sms ? (int)total : g_num_sms;
+  if (epi == EPI_SPLIT_DET) {
+    const long long tiles = total / p.split_k;
+    if (tiles * 4 > (long long)DET_COUNTER_BYTES) return set_error("bb_gemm_bf16: too many output tiles for deterministic split-K");
+    p.det_part = det_partials(stream, (size_t)total * BLOCK_M * bn * sizeof(float), "bb_gemm_bf16 (split-K)");
+    if (!p.det_part) return -1;
+    p.det_cnt = det_counters(stream);
+  }
   if (g_prof_on && g_prof_buf && g_prof_used < g_prof_cap) {
     if (g_prof_used == g_prof.size()) g_prof.push_back(ProfRec());
     ProfRec* rec = &g_prof[g_prof_used];

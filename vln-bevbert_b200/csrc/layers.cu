@@ -91,6 +91,7 @@ static inline char* at(void* base, int64_t off) { return reinterpret_cast<char*>
 // everything enqueued on `main` so far; the caller joins once after backward (bb_side_join) and keeps the buffers those
 // kernels read alive until then.  Inside a CUDA-graph capture this becomes a fork / join of the graph.
 static cudaStream_t g_side = nullptr;
+cudaStream_t side_stream() { return g_side; }
 static cudaEvent_t g_fork_ev[32];
 static int g_fork_i = 0;
 static bool g_side_used = false;

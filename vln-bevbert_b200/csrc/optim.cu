@@ -44,7 +44,7 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 }
 
 __global__ void __launch_bounds__(MT_THREADS) mt_sumsq_kernel(const bb_mt_tensor* __restrict__ table, int nt,
-                                                             float* __restrict__ out) {
+                                                             float* __restrict__ out, float* __restrict__ det_part) {
   __shared__ float sh[MT_THREADS / 32];
   bb::pdl_wait();
   bb::pdl_trigger();
@@ -69,7 +69,23 @@ __global__ void __launch_bounds__(MT_THREADS) mt_sumsq_kernel(const bb_mt_tensor
     for (long long i = base + threadIdx.x; i < n && i < base + MT_CHUNK; i += MT_THREADS) acc += g[i] * g[i];
   }
   const float s = block_sum(acc, sh);
-  if (threadIdx.x == 0) atomicAdd(out, s);
+  if (threadIdx.x == 0) {
+    if (det_part) det_part[chunk] = s;   // deterministic mode: summed in chunk order by mt_sumsq_det_kernel
+    else atomicAdd(out, s);
+  }
+}
+
+// Deterministic mode: one block sums the per-chunk partials; thread t adds chunks t, t + MT_THREADS, ... in order, and
+// block_sum combines the threads in a fixed tree.
+__global__ void __launch_bounds__(MT_THREADS) mt_sumsq_det_kernel(const float* __restrict__ part, long long n,
+                                                                 float* __restrict__ out) {
+  __shared__ float sh[MT_THREADS / 32];
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  float acc = 0.f;
+  for (long long i = threadIdx.x; i < n; i += MT_THREADS) acc += part[i];
+  const float s = block_sum(acc, sh);
+  if (threadIdx.x == 0) *out = s;
 }
 
 struct AdamParams {
@@ -184,9 +200,18 @@ extern "C" int bb_mt_sumsq(const bb_mt_tensor* table_dev, int ntensors, int64_t 
   if (cudaMemsetAsync(out, 0, sizeof(float), s) != cudaSuccess) return set_error("bb_mt_sumsq: memset failed");
   if (ntensors <= 0 || total_chunks <= 0) return 0;
   if (total_chunks > 0x7fffffffLL) return set_error("bb_mt_sumsq: too many chunks");
-  bb::launch_pdl(mt_sumsq_kernel, (unsigned)total_chunks, MT_THREADS, 0, s, table_dev, ntensors, out);
+  float* part = nullptr;
+  if (det_on()) {
+    part = det_partials(s, (size_t)total_chunks * sizeof(float), "bb_mt_sumsq");
+    if (!part) return -1;
+  }
+  bb::launch_pdl(mt_sumsq_kernel, (unsigned)total_chunks, MT_THREADS, 0, s, table_dev, ntensors, out, part);
   count_launch();
-  return check_launch("mt_sumsq_kernel");
+  if (int e = check_launch("mt_sumsq_kernel")) return e;
+  if (!part) return 0;
+  bb::launch_pdl(mt_sumsq_det_kernel, 1, MT_THREADS, 0, s, (const float*)part, (long long)total_chunks, out);
+  count_launch();
+  return check_launch("mt_sumsq_det_kernel");
 }
 
 extern "C" int bb_adamw_step(const bb_mt_tensor* table_dev, int ntensors, int64_t total_chunks, float beta1, float beta2,

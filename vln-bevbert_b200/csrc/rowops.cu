@@ -2,7 +2,8 @@
 // (dropout + residual +) LayerNorm forward/backward, masked softmax forward/backward with the graph bias,
 // bias-gradient column sums, embedding sum / scatter, row gather / scatter-add and fused softmax
 // cross-entropy. One warp per row where rows are <= 1024 wide, 16-byte vector accesses, fp32 math,
-// bf16 storage, warp-shuffle reductions; parameter-gradient reductions use per-block partials + atomics.
+// bf16 storage, warp-shuffle reductions; parameter-gradient reductions use per-block partials + atomics, or, in the
+// deterministic mode, per-block partials in a workspace summed in block order by a second kernel (det_reduce).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -393,7 +394,7 @@ layernorm_bwd_kernel(const DYT* __restrict__ dy, const XT* __restrict__ x, const
                      const float* __restrict__ rstd_in, long long rows, int H, uint64_t seed_in, uint32_t thresh_in,
                      float scale_in, uint64_t seed_out, uint32_t thresh_out, float scale_out, DXT* __restrict__ dx,
                      T* __restrict__ dres, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                     float* __restrict__ dxsum) {
+                     float* __restrict__ dxsum, float* __restrict__ det_part) {
   bb::pdl_wait();
   bb::pdl_trigger();
   extern __shared__ float ln_part[];  // [3][LN_WARPS][H] per-warp partial dgamma / dbeta / dxsum
@@ -516,6 +517,13 @@ layernorm_bwd_kernel(const DYT* __restrict__ dy, const XT* __restrict__ x, const
         b += sb[w * H + i];
         x_ += sx[w * H + i];
       }
+      if (det_part) {   // deterministic mode: this block's partials, summed in block order by det_reduce
+        float* pp = det_part + (long long)blockIdx.x * 3 * H;
+        pp[i] = a;
+        pp[H + i] = b;
+        pp[2 * H + i] = x_;
+        continue;
+      }
       if (dgamma) atomicAdd(dgamma + i, a);
       if (dbeta) atomicAdd(dbeta + i, b);
       if (dxsum) atomicAdd(dxsum + i, x_);
@@ -526,7 +534,8 @@ layernorm_bwd_kernel(const DYT* __restrict__ dy, const XT* __restrict__ x, const
 // ------------------------------------------------------------------------------------- column sums
 template <typename T>
 __global__ void __launch_bounds__(256)
-colsum_bf16_kernel(const T* __restrict__ x, long long rows, int N, long long ld, float* __restrict__ out) {
+colsum_bf16_kernel(const T* __restrict__ x, long long rows, int N, long long ld, float* __restrict__ out,
+                   float* __restrict__ det_part) {
   bb::pdl_wait();
   bb::pdl_trigger();
   // blockDim = (32, 8): 32 lanes x 8 columns each = 256 columns per block in x; rows strided over y and grid.y
@@ -570,7 +579,26 @@ colsum_bf16_kernel(const T* __restrict__ x, long long rows, int N, long long ld,
 #pragma unroll
   for (int yy = 0; yy < 8; ++yy) s += part[yy][t];
   const int c = blockIdx.x * 256 + t;
-  if (c < N) atomicAdd(out + c, s);
+  if (c >= N) return;
+  if (det_part) det_part[(long long)blockIdx.y * N + c] = s;   // deterministic mode: summed by det_reduce
+  else atomicAdd(out + c, s);
+}
+
+// o_k[i] += sum of the partials part[p][k][i] over p in ascending order (see common.h)
+__global__ void det_reduce_kernel(const float* __restrict__ part, int nparts, long long n, int nout, float* o0,
+                                  float* o1, float* o2) {
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n * nout; i += stride) {
+    const int k = (int)(i / n);
+    const long long e = i - (long long)k * n;
+    float* o = k == 0 ? o0 : (k == 1 ? o1 : o2);
+    if (!o) continue;
+    float s = part[i];
+    for (int p = 1; p < nparts; ++p) s += part[(long long)p * nout * n + i];
+    o[e] += s;
+  }
 }
 
 // ------------------------------------------------------------------------------------- softmax
@@ -635,7 +663,7 @@ template <int MAXE, typename T>
 __global__ void __launch_bounds__(256)
 softmax_bwd_kernel(const T* __restrict__ probs, const float* __restrict__ dprobs, long long nrows, int H, int nq,
                    int nk, int ld, uint64_t seed, uint32_t thresh, float scale, float out_scale, T* __restrict__ ds,
-                   float* __restrict__ dbias) {
+                   float* __restrict__ dbias, long long dbias_hs) {
   bb::pdl_wait();
   bb::pdl_trigger();
   const int lane = threadIdx.x & 31;
@@ -662,14 +690,18 @@ softmax_bwd_kernel(const T* __restrict__ probs, const float* __restrict__ dprobs
   }
   dot = warp_sum(dot);
   T* o = ds + row * ld;
-  float* db = dbias ? dbias + (b * nq + q) * nk : nullptr;
+  // dbias_hs != 0 (deterministic mode): per-head partials dbias[h] at a stride of dbias_hs, one plain store each
+  float* db = dbias ? dbias + (dbias_hs ? (row / nq % H) * dbias_hs : 0) + (b * nq + q) * nk : nullptr;
 #pragma unroll
   for (int e = 0; e < MAXE; ++e) {
     const int k = e * 32 + lane;
     if (k < ld) {
       const float d = (k < nk) ? pv[e] * (g[e] - dot) : 0.f;
       o[k] = fromf<T>(d * out_scale);
-      if (db && k < nk) atomicAdd(db + k, d);
+      if (db && k < nk) {
+        if (dbias_hs) db[k] = d;
+        else atomicAdd(db + k, d);
+      }
     }
   }
 }
@@ -740,6 +772,42 @@ __global__ void scatter_add_rows_kernel(const T* __restrict__ in, const int64_t*
   const int c = i % H;
   const int64_t dst = idx[r];
   if (dst >= 0) atomicAdd(out + dst * H + c, tof(in[i]));
+}
+// Deterministic scatter-add by destination: entries e = 0 .. n-1 are sorted by destination dst[e] (stably, so equal
+// destinations keep ascending source order); out[d] += ((t_e1 + t_e2) + ...) over the run of entries with dst == d,
+// t_e = w[e] * src[src_row[e]] (one rounded product, no FMA) or src[src_row[e]] without w.  dst < 0 is dropped.  The
+// thread of a run's first entry walks the run, 8 columns at a time.
+template <typename S>
+__global__ void scatter_rows_sorted_kernel(const S* __restrict__ src, const int64_t* __restrict__ src_row,
+                                           const float* __restrict__ w, const int64_t* __restrict__ dst, long long n,
+                                           int H, float* __restrict__ out) {
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  const int h8 = H / 8;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= n * h8) return;
+  const long long e0 = i / h8;
+  const int c = (int)(i % h8) * 8;
+  const int64_t d = dst[e0];
+  if (d < 0 || (e0 > 0 && dst[e0 - 1] == d)) return;
+  float acc[8];
+  for (long long e = e0; e < n && dst[e] == d; ++e) {
+    float v[8];
+    load8(src + src_row[e] * H + c, v);
+    if (w) {
+      const float ww = w[e];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = __fmul_rn(ww, v[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = e == e0 ? v[j] : __fadd_rn(acc[j], v[j]);
+  }
+  float o[8];
+  float* po = out + d * H + c;
+  load8(po, o);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = __fadd_rn(o[j], acc[j]);
+  store8(po, o);
 }
 
 // ------------------------------------------------------------------------------------- softmax cross entropy
@@ -899,6 +967,7 @@ extern "C" int bb_segment_wsum_bwd(const void* dout, const int32_t* seg_off, con
                                    int64_t nseg, int H, float* dsrc_f32, void* stream) {
   if (nseg <= 0) return 0;
   if (H % 8 != 0) return set_error("bb_segment_wsum_bwd: H must be a multiple of 8");
+  if (det_on()) return set_error("bb_segment_wsum_bwd adds with atomics; in deterministic mode use bb_scatter_rows_sorted");
   ACT_T(bb::launch_pdl(segment_wsum_bwd_kernel<T>, (unsigned)((nseg + 7) / 8), 256, 0, STREAM, (const T*)dout, seg_off, idx, w, nseg, H,
                                                                           dsrc_f32));
   count_launch();
@@ -941,6 +1010,11 @@ extern "C" int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x
   if (g > device_sms()) g = device_sms();   // one resident block per SM (233 registers), rows grid-strided
   const unsigned grid = (unsigned)g;
   const size_t ln_smem = (size_t)3 * LN_WARPS * H * sizeof(float);
+  float* part = nullptr;
+  if (det_on() && (dgamma || dbeta || dxsum)) {
+    part = det_partials(STREAM, (size_t)grid * 3 * H * sizeof(float), "bb_layernorm_bwd");
+    if (!part) return -1;
+  }
 #define LN_BWD(DYT, XT, DXT, AT)                                                                                    \
   do {                                                                                                              \
     static bool attr_done = false;                                                                                  \
@@ -952,11 +1026,11 @@ extern "C" int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x
     if (H <= 768)                                                                                                   \
       bb::launch_pdl(layernorm_bwd_kernel<DYT, XT, DXT, AT, 3>, grid, LN_WARPS * 32, ln_smem, STREAM, (const DYT*)dy, \
                      (const XT*)x, (const AT*)residual, gamma, mean, rstd, rows, H, seed_in, thresh_in, scale_in,   \
-                     seed_out, thresh_out, scale_out, (DXT*)dx, (AT*)dres, dgamma, dbeta, dxsum);                   \
+                     seed_out, thresh_out, scale_out, (DXT*)dx, (AT*)dres, dgamma, dbeta, dxsum, part);             \
     else                                                                                                            \
       bb::launch_pdl(layernorm_bwd_kernel<DYT, XT, DXT, AT, 4>, grid, LN_WARPS * 32, ln_smem, STREAM, (const DYT*)dy, \
                      (const XT*)x, (const AT*)residual, gamma, mean, rstd, rows, H, seed_in, thresh_in, scale_in,   \
-                     seed_out, thresh_out, scale_out, (DXT*)dx, (AT*)dres, dgamma, dbeta, dxsum);                   \
+                     seed_out, thresh_out, scale_out, (DXT*)dx, (AT*)dres, dgamma, dbeta, dxsum, part);             \
   } while (0)
   if (bb::act_f32()) {
     if (dy_f32 && x_f32 && dx_f32) LN_BWD(float, float, float, float);
@@ -970,17 +1044,41 @@ extern "C" int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x
   else return set_error("bb_layernorm_bwd: unsupported dtype combination");
 #undef LN_BWD
   count_launch();
-  return check_launch("layernorm_bwd_kernel");
+  if (int e = check_launch("layernorm_bwd_kernel")) return e;
+  return part ? det_reduce(part, (int)grid, H, 3, dgamma, dbeta, dxsum, STREAM) : 0;
 }
 
-extern "C" int bb_colsum_bf16(const void* x, int64_t rows, int N, int64_t ld, float* out, void* stream) {
+namespace bb {
+template <typename T>
+static int colsum_run(const T* x, long long rows, int N, long long ld, float* out, cudaStream_t stream) {
   if (rows <= 0 || N <= 0) return 0;
   long long gy = (rows + 63) / 64;
   if (gy > 64) gy = 64;
   dim3 grid((N + 255) / 256, (unsigned)gy);
-  ACT_T(bb::launch_pdl(colsum_bf16_kernel<T>, grid, dim3(32, 8), 0, STREAM, (const T*)x, rows, N, ld, out));
+  float* part = nullptr;
+  if (det_on()) {
+    part = det_partials(stream, (size_t)gy * N * sizeof(float), "bb_colsum_bf16");
+    if (!part) return -1;
+  }
+  bb::launch_pdl(colsum_bf16_kernel<T>, grid, dim3(32, 8), 0, stream, x, rows, N, ld, out, part);
   count_launch();
-  return check_launch("colsum_bf16_kernel");
+  if (int e = check_launch("colsum_bf16_kernel")) return e;
+  return part ? det_reduce(part, (int)gy, N, 1, out, nullptr, nullptr, stream) : 0;
+}
+
+int det_reduce(const float* part, int nparts, long long n, int nout, float* o0, float* o1, float* o2,
+               cudaStream_t stream) {
+  if (n <= 0 || nparts <= 0) return 0;
+  bb::launch_pdl(det_reduce_kernel, grid1d(n * nout, 256), 256, 0, stream, part, nparts, n, nout, o0, o1, o2);
+  count_launch();
+  return check_launch("det_reduce_kernel");
+}
+}  // namespace bb
+
+extern "C" int bb_colsum_bf16(const void* x, int64_t rows, int N, int64_t ld, float* out, void* stream) {
+  int rc = 0;
+  ACT_T(rc = colsum_run((const T*)x, rows, N, ld, out, STREAM));
+  return rc;
 }
 
 extern "C" int bb_softmax_fwd(const float* scores, const float* kmask, const float* bias, int nbatch, int H, int nq,
@@ -1010,17 +1108,25 @@ extern "C" int bb_softmax_bwd(const void* probs, const float* dprobs, int nbatch
   if (nrows <= 0) return 0;
   if (ld < nk || ld > 1024) return set_error("bb_softmax_bwd: need nk <= ld <= 1024");
   const unsigned grid = (unsigned)((nrows + 7) / 8);
+  float* dbias_out = dbias;
+  long long hs = 0;   // deterministic mode: per-head bias-gradient partials, then a sum over heads in head order
+  if (dbias && det_on()) {
+    hs = (long long)nbatch * nq * nk;
+    dbias = det_partials(STREAM, (size_t)H * hs * sizeof(float), "bb_softmax_bwd (graph-bias gradient)");
+    if (!dbias) return -1;
+  }
   if (ld <= 128)
     ACT_T(bb::launch_pdl(softmax_bwd_kernel<4, T>, grid, 256, 0, STREAM, (const T*)probs, dprobs, nrows, H, nq, nk, ld, seed, thresh,
-                                                    scale, out_scale, (T*)ds, dbias));
+                                                    scale, out_scale, (T*)ds, dbias, hs));
   else if (ld <= 512)
     ACT_T(bb::launch_pdl(softmax_bwd_kernel<16, T>, grid, 256, 0, STREAM, (const T*)probs, dprobs, nrows, H, nq, nk, ld, seed, thresh,
-                                                     scale, out_scale, (T*)ds, dbias));
+                                                     scale, out_scale, (T*)ds, dbias, hs));
   else
     ACT_T(bb::launch_pdl(softmax_bwd_kernel<32, T>, grid, 256, 0, STREAM, (const T*)probs, dprobs, nrows, H, nq, nk, ld, seed, thresh,
-                                                     scale, out_scale, (T*)ds, dbias));
+                                                     scale, out_scale, (T*)ds, dbias, hs));
   count_launch();
-  return check_launch("softmax_bwd_kernel");
+  if (int e = check_launch("softmax_bwd_kernel")) return e;
+  return hs ? det_reduce(dbias, H, hs, 1, dbias_out, nullptr, nullptr, STREAM) : 0;
 }
 
 extern "C" int bb_embed_sum(const int64_t* ids, const float* word, const float* pos, const float* type0, int64_t ntok,
@@ -1035,6 +1141,17 @@ extern "C" int bb_embed_sum(const int64_t* ids, const float* word, const float* 
 extern "C" int bb_embed_scatter_grad(const int64_t* ids, const float* dz, int64_t ntok, int L, int H,
                                      int64_t padding_idx, float* dword, float* dpos, float* dtype0, void* stream) {
   if (ntok <= 0) return 0;
+  if (det_on()) {
+    // word table: by destination through bb_scatter_rows_sorted; position table: dpos[l] += sum over b, in b order, of
+    // dz[b, l]; type row: a column sum
+    if (dword) return set_error("bb_embed_scatter_grad: in deterministic mode the word-table gradient goes through "
+                                "bb_scatter_rows_sorted (pass dword = NULL)");
+    if (dpos && ntok % L) return set_error("bb_embed_scatter_grad: ntok must be a multiple of L");
+    if (dpos) {
+      if (int e = det_reduce(dz, (int)(ntok / L), (long long)L * H, 1, dpos, nullptr, nullptr, STREAM)) return e;
+    }
+    return dtype0 ? colsum_run(dz, ntok, H, H, dtype0, STREAM) : 0;
+  }
   const long long n = ntok * H;
   bb::launch_pdl(embed_scatter_grad_kernel, (unsigned)((n + 255) / 256), 256, 0, STREAM, ids, dz, ntok, L, H, padding_idx, dword,
                                                                              dpos, dtype0);
@@ -1053,10 +1170,31 @@ extern "C" int bb_gather_rows_bf16(const void* in, const int64_t* idx, int64_t n
 extern "C" int bb_scatter_add_rows(const void* in_bf16, const int64_t* idx, int64_t nin, int H, float* out_f32,
                                    void* stream) {
   if (nin <= 0) return 0;
+  if (det_on()) return set_error("bb_scatter_add_rows adds with atomics; in deterministic mode use bb_scatter_rows_sorted");
   const long long n = nin * H;
   ACT_T(bb::launch_pdl(scatter_add_rows_kernel<T>, (unsigned)((n + 255) / 256), 256, 0, STREAM, (const T*)in_bf16, idx, nin, H, out_f32));
   count_launch();
   return check_launch("scatter_add_rows_kernel");
+}
+
+extern "C" int bb_scatter_rows_sorted(const void* src, int src_f32, const int64_t* src_row, const float* w,
+                                      const int64_t* dst_sorted, int64_t n, int H, float* out_f32, void* stream) {
+  if (n <= 0) return 0;
+  if (H % 8 != 0) return set_error("bb_scatter_rows_sorted: H must be a multiple of 8");
+  if ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(out_f32)) & 15)
+    return set_error("bb_scatter_rows_sorted: src and out must be 16-byte aligned");
+  const long long nt = n * (H / 8);
+  const unsigned grid = (unsigned)((nt + 255) / 256);
+  if (src_f32)
+    bb::launch_pdl(scatter_rows_sorted_kernel<float>, grid, 256, 0, STREAM, (const float*)src, src_row, w, dst_sorted,
+                   n, H, out_f32);
+  else if (bb::act_f32())
+    return set_error("bb_scatter_rows_sorted: the fp32 verification mode needs fp32 src");
+  else
+    bb::launch_pdl(scatter_rows_sorted_kernel<bf16>, grid, 256, 0, STREAM, (const bf16*)src, src_row, w, dst_sorted,
+                   n, H, out_f32);
+  count_launch();
+  return check_launch("scatter_rows_sorted_kernel");
 }
 
 extern "C" int bb_softmax_xent(const float* logits, const int64_t* labels, int64_t rows, int V, int64_t ld, float* loss,

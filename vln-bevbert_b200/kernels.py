@@ -6,6 +6,7 @@ functions raise.  (tests/emu_kernels.py replaces this module's functions with to
 exercise the host-side block logic on CPU; that emulation is test infrastructure, never shipped.)
 """
 import ctypes as C
+import warnings
 
 import torch
 
@@ -50,10 +51,68 @@ _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
 
 
 def _stream():
-    """raw cudaStream_t of torch's current stream on the current device (fast path avoids building a Stream object)."""
+    """raw cudaStream_t of torch's current stream on the current device (fast path avoids building a Stream object).
+    Every launch asks for it, so this is also where the library's deterministic mode follows torch's flag."""
+    if _det_mode() != _DET_MODE:
+        _set_det_mode(_det_mode())
     if _raw_stream is not None:
         return _raw_stream(torch.cuda.current_device())
     return torch.cuda.current_stream().cuda_stream
+
+
+# ---------------------------------------------------------------------------------------------- deterministic mode
+# torch.use_deterministic_algorithms(True) switches the library to fixed-order reductions (bb_set_deterministic):
+# bit-identical results for bit-identical inputs on the same build and GPU model.  warn_only=True maps to mode 2, in
+# which the one path without a deterministic kernel runs after a warning instead of raising.
+DET_WS_BYTES = 32 << 20     # per stream; the largest user is a split-K weight gradient at about one wave of tiles
+_DET_MODE = 0
+_DET_WS = None
+
+
+def _det_mode():
+    if not torch._C._get_deterministic_algorithms():
+        return 0
+    return 2 if torch._C._get_deterministic_algorithms_warn_only() else 1
+
+
+def _set_det_mode(mode):
+    """Registers the zero-filled main / side workspaces before the first deterministic launch (they stay allocated at
+    fixed addresses, so a CUDA graph captured later can use them), then sets the library's mode."""
+    global _DET_MODE, _DET_WS
+    lib = _lib.load()
+    if mode and _DET_WS is None:
+        if _capturing():
+            raise RuntimeError("deterministic mode was switched on during a CUDA-graph capture; call "
+                               "torch.use_deterministic_algorithms(True) and run one eager step before capturing")
+        _DET_WS = [torch.zeros(DET_WS_BYTES, dtype=torch.uint8, device="cuda") for _ in range(2)]
+        torch.cuda.synchronize()
+        _lib.check(lib.bb_set_det_workspace(_DET_WS[0].data_ptr(), _DET_WS[1].data_ptr(), DET_WS_BYTES),
+                   "bb_set_det_workspace")
+    _lib.check(lib.bb_set_deterministic(mode), "bb_set_deterministic")
+    _DET_MODE = mode
+
+
+def _nondeterministic(what):
+    """torch's contract for a path without a deterministic implementation: raise under the flag, or warn with
+    warn_only=True."""
+    mode = _det_mode()
+    if mode == 1:
+        raise RuntimeError("%s does not have a deterministic implementation, but torch.use_deterministic_algorithms"
+                           "(True) is set" % what)
+    if mode == 2:
+        warnings.warn("%s does not have a deterministic implementation" % what)
+
+
+def _scatter_sorted(src, dst, H, out_f32, src_row=None, w=None):
+    """out_f32[dst[e]] += ((t_e1 + t_e2) + ...) in ascending source order e, t_e = (w[e] *) src[src_row[e] | e];
+    dst < 0 is dropped (bb_scatter_rows_sorted after a stable sort of the destinations)."""
+    keys, perm = torch.sort(dst, stable=True)
+    rows = perm if src_row is None else src_row[perm]
+    wp = w[perm].contiguous() if w is not None else None
+    _lib.check(_lib.load().bb_scatter_rows_sorted(src.data_ptr(), int(src.dtype == torch.float32), rows.data_ptr(),
+                                                  _p(wp), keys.data_ptr(), keys.numel(), H, out_f32.data_ptr(),
+                                                  _stream()), "bb_scatter_rows_sorted")
+    return out_f32
 
 
 def _req(t, dtype, name):
@@ -198,6 +257,9 @@ def sublayer_fwd(d):
 
 def sublayer_bwd(d):
     lib = _lib.load()
+    if (isinstance(d, _lib.AttnDesc) and d.want_dbias and not FLASH and d.Hd // d.heads == 64
+            and d.nk <= FUSED_SCORES_MAX_KEYS):
+        _nondeterministic("the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient")
     fn = {_lib.AttnDesc: lib.bb_attn_bwd, _lib.FfnDesc: lib.bb_ffn_bwd, _lib.PanoDesc: lib.bb_pano_bwd}[type(d)]
     _lib.check(fn(C.byref(d), _stream()), "bb_sublayer_bwd")
 
@@ -225,6 +287,8 @@ def attn_scores_fwd(q, ldq, k, ldk, B, H, nq, nk, dh, ldp, kmask, bias, drop):
 def attn_scores_bwd(dctx, ldd, v, ldv, P, B, H, nq, nk, dh, ldp, drop, dbias=None):
     """fused dS = P o (g - sum P g) / sqrt(dh), g = dropout-mask(dctx V^T): -> dS bf16 (B,H,nq,ldp)."""
     lib = _lib.load()
+    if dbias is not None:
+        _nondeterministic("the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient")
     a = _lib.AttnScoresArgs()
     a.A, a.lda, a.a_s1, a.a_s2 = dctx.data_ptr(), ldd, dh, nq * ldd
     a.Bm, a.ldb, a.b_s1, a.b_s2 = v.data_ptr(), ldv, dh, nk * ldv
@@ -472,6 +536,11 @@ def embed_sum(ids, word, pos, type0):
 def embed_scatter_grad(ids, dz, L, padding_idx, dword, dpos, dtype0):
     lib = _lib.load()
     ntok, H = dz.shape
+    if torch.are_deterministic_algorithms_enabled() and dword is not None:
+        # the word table by destination here; the library sums the position and type tables in a fixed order
+        ids1 = ids.reshape(-1)
+        _scatter_sorted(dz, torch.where(ids1 == padding_idx, -1, ids1), H, dword)
+        dword = None
     _lib.check(lib.bb_embed_scatter_grad(ids.contiguous().data_ptr(), dz.data_ptr(), ntok, L, H, padding_idx,
                                          _p(dword), _p(dpos), _p(dtype0), _stream()), "bb_embed_scatter_grad")
 
@@ -487,6 +556,8 @@ def gather_rows(src, idx, H):
 
 def scatter_add_rows(src, idx, H, out_f32):
     """out_f32[idx[r]] += src[r]."""
+    if torch.are_deterministic_algorithms_enabled():
+        return _scatter_sorted(src, idx.reshape(-1), H, out_f32)
     lib = _lib.load()
     _lib.check(lib.bb_scatter_add_rows(src.data_ptr(), idx.data_ptr(), idx.numel(), H, out_f32.data_ptr(), _stream()),
                "bb_scatter_add_rows")
@@ -536,6 +607,12 @@ def segment_wsum(src, seg_off, idx, w, nseg, H):
 
 
 def segment_wsum_bwd(dout, seg_off, idx, w, nseg, H, dsrc_f32):
+    if torch.are_deterministic_algorithms_enabled():
+        # by destination: entry e of segment s adds w[e] * dout[s] to dsrc[idx[e]]
+        e = torch.arange(idx.numel(), dtype=seg_off.dtype, device=idx.device)
+        seg = torch.searchsorted(seg_off, e, right=True) - 1
+        dst = torch.where((seg >= 0) & (seg < nseg), idx.long(), -1)
+        return _scatter_sorted(dout, dst, H, dsrc_f32, src_row=seg.clamp(0, max(nseg - 1, 0)), w=w)
     lib = _lib.load()
     _lib.check(lib.bb_segment_wsum_bwd(dout.data_ptr(), seg_off.data_ptr(), idx.data_ptr(), w.data_ptr(), nseg, H,
                                        dsrc_f32.data_ptr(), _stream()), "bb_segment_wsum_bwd")
