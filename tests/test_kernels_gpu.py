@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import emu_kernels as E
+from drop_masks import ln_keep as _ln_keep_mask
 from helpers import rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -148,29 +149,6 @@ def test_layernorm_fwd_bwd(K, x_f32, res):
         assert rel_l2(dres, rdres) < 6e-3
     assert rel_l2(dg, rdg) < 1e-4 and rel_l2(db, rdb) < 1e-4
     assert float((dxs.cpu() - rdx.sum(0)).norm()) < 1e-3 * float(rdx.abs().sum(0).norm())   # bias grad of the dense before LN
-
-
-def _ln_keep_mask(seed, rows, H, thresh):
-    """torch restatement of the LayerNorm-site dropout decisions (csrc/rowops.cu ln_keep8: one hash per 8-element vector,
-    four mixes, 16-bit halves), for checking that forward and backward apply the documented function."""
-    M = 0xFFFFFFFF
-    vec = torch.arange(rows * H // 8, dtype=torch.int64)
-    x = (vec & M) ^ (((vec >> 32) * 0x9E3779B1) & M) ^ (seed & M) ^ (((seed >> 32) * 0x85EBCA6B) & M)
-    x = x ^ (x >> 16)
-    x = (x * 0x7FEB352D) & M
-    x = x ^ (x >> 15)
-    x = (x * 0x846CA68B) & M
-    h = x ^ (x >> 16)
-    t16 = thresh >> 16
-    keep = torch.zeros(rows * H // 8, 8, dtype=torch.bool)
-    for k in range(4):
-        y = (h + (k + 1) * 0x9E3779B1) & M
-        y = y ^ (y >> 15)
-        y = (y * 0x2C1B3C6D) & M
-        y = y ^ (y >> 16)
-        keep[:, 2 * k] = (y & 0xFFFF) >= t16
-        keep[:, 2 * k + 1] = (y >> 16) >= t16
-    return keep.reshape(rows, H)
 
 
 def test_layernorm_dropout_replay(K):
