@@ -1,5 +1,6 @@
 // Batched bf16 GEMM for sm_90a: TMA -> 128B-swizzled shared memory -> wgmma (fp32 accumulators in registers) ->
-// register epilogue with fused bias / GELU / ReLU / gelu' / dropout / residual.
+// epilogue with fused bias / GELU / ReLU / gelu' / dropout / residual, staged through shared memory so that global
+// accesses are 16-byte row segments and the per-element code is one compact loop.
 //
 // Persistent, warp-specialised, ping-pong: warpgroup 0 is the TMA producer (one lane issues), warpgroups 1 and 2 are
 // consumers that each own whole output tiles and alternate over the CTA's tile sequence.  The two consumers take turns
@@ -114,145 +115,231 @@ __device__ __forceinline__ bool epi_add_of(const GemmKParams& p) {
   return EPI == EPI_GENERIC ? p.add_in != nullptr : EPI == EPI_ADD;
 }
 
-// Epilogue of two adjacent output columns (col, col + 1) of one row at element offset `off`; col is even.  b0 / b1 are
-// the bias of the two columns (added when add_bias), mul_in / add_v the aux_in and add_in values of the pair, all read
-// by the caller.  EDGE: the pair may straddle the last column or lack the alignment of a paired store.
-template <int EPI, bool EDGE>
-__device__ __forceinline__ void epi_pair(const GemmKParams& p, long long off, int col, float v0, float v1,
-                                         bool add_bias, float b0, float b1, __nv_bfloat162 mul_in,
-                                         __nv_bfloat162 add_v) {
-  const bool two = !EDGE || col + 1 < p.N;
-  const bool vec = !EDGE || (two && p.vec_ok);
-  const bool generic = EPI == EPI_GENERIC;
-  const bool aux_out = generic ? p.aux_out != nullptr : EPI == EPI_GELU_PRE;
-  const int act = generic ? p.act : (EPI == EPI_GELU_PRE ? 1 : 0);
-  const int mul = epi_mul_of<EPI>(p);
-  const bool drop = (generic || EPI >= EPI_GELU_PRE) && p.drop_thresh != 0;
-  const bool out_f32 = EPI == EPI_ATOMIC || ((generic || EPI == EPI_PLAIN) && p.out_f32 != 0);
-  const bool atomic = EPI == EPI_ATOMIC || (generic && p.atomic != 0);
-  const bool fast_gelu = generic && p.fast_gelu;
-  v0 *= p.alpha;
-  v1 *= p.alpha;
-  if (add_bias) {
-    v0 += b0;
-    if (two) v1 += b1;
-  }
-  if (aux_out) {
-    if (vec) *reinterpret_cast<__nv_bfloat162*>(p.aux_out + off) = __floats2bfloat162_rn(v0, v1);
-    else {
-      p.aux_out[off] = __float2bfloat16(v0);
-      if (two) p.aux_out[off + 1] = __float2bfloat16(v1);
-    }
-  }
-  if (act == 1) {
-    if (fast_gelu) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
-    else { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-  } else if (act == 2) {
-    v0 = fmaxf(v0, 0.0f);
-    v1 = fmaxf(v1, 0.0f);
-  }
-  if (mul != 0) {
-    const float2 a = __bfloat1622float2(mul_in);
-    if (mul == 1) {
-      if (fast_gelu) { v0 *= dgelu_fast(a.x); v1 *= dgelu_fast(a.y); }
-      else { v0 *= dgelu_erf(a.x); v1 *= dgelu_erf(a.y); }
-    } else {
-      v0 = a.x > 0.0f ? v0 : 0.0f;
-      v1 = a.y > 0.0f ? v1 : 0.0f;
-    }
-  }
-  if (drop) {
-    v0 = drop_keep(p.drop_seed, (uint64_t)off, p.drop_thresh) ? v0 * p.drop_scale : 0.0f;
-    v1 = drop_keep(p.drop_seed, (uint64_t)(off + 1), p.drop_thresh) ? v1 * p.drop_scale : 0.0f;
-  }
-  if (epi_add_of<EPI>(p)) {
-    const float2 a = __bfloat1622float2(add_v);
-    v0 += a.x;
-    if (two) v1 += a.y;
-  }
-  if (out_f32) {
-    float* D = reinterpret_cast<float*>(p.D) + off;
-    if (atomic) {
+// Epilogues of EPI_ATOMIC (split-K weight gradients) and EPI_SPLIT_DET read the accumulators straight from registers;
+// every other variant stages them through shared memory (epilogue_staged).
+__host__ __device__ constexpr bool epi_staged(int epi) { return epi != EPI_ATOMIC && epi != EPI_SPLIT_DET; }
+// Shared memory of the two staging buffers (64 x BN fp32 each), carved out ahead of the stage ring.
+__host__ __device__ constexpr int staging_bytes(int bn, int epi) { return epi_staged(epi) ? 2 * 64 * bn * 4 : 0; }
+
+// Epilogue of EPI_ATOMIC for one 128 x BN tile: alpha, bias, fp32 atomic add of each accumulator pair straight from
+// registers.  acc[hh] holds rows 64 hh .. 64 hh + 63 in the wgmma fragment order (thread rows r0, r0 + 8; columns
+// 8 j + cq, + 1).  EDGE: the tile may extend past the last row or column, or lack paired-access alignment.
+template <int BN, bool EDGE>
+__device__ __forceinline__ void epilogue_atomic(const GemmKParams& p, const TileCoord& t, const float (&acc)[2][BN / 2],
+                                                int r0, int cq) {
+  const int n0 = t.n_tile * BN;
+  const bool add_bias = p.bias != nullptr && t.split == 0;
+  const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + cq;
+    if (EDGE && col >= p.N) continue;
+    const bool two = !EDGE || col + 1 < p.N;
+    const bool vec = !EDGE || (two && p.vec_ok);
+    const float b0 = add_bias ? __ldg(p.bias + col) : 0.0f;
+    const float b1 = add_bias && two ? __ldg(p.bias + col + 1) : 0.0f;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int hh = r >> 1, h = r & 1;
+      const int row = t.m_tile * BLOCK_M + 64 * hh + r0 + 8 * h;
+      if (EDGE && row >= p.M) continue;
+      float* D = reinterpret_cast<float*>(p.D) + batch_off + (long long)row * p.ldd + col;
+      float v0 = acc[hh][4 * j + 2 * h] * p.alpha, v1 = acc[hh][4 * j + 2 * h + 1] * p.alpha;
+      if (add_bias) {
+        v0 += b0;
+        if (two) v1 += b1;
+      }
       if (vec) {
         atomicAdd(reinterpret_cast<float2*>(D), make_float2(v0, v1));
       } else {
         atomicAdd(D, v0);
         if (two) atomicAdd(D + 1, v1);
       }
-    } else if (vec) {
-      *reinterpret_cast<float2*>(D) = make_float2(v0, v1);
-    } else {
-      D[0] = v0;
-      if (two) D[1] = v1;
-    }
-  } else {
-    __nv_bfloat16* D = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
-    if (vec) *reinterpret_cast<__nv_bfloat162*>(D) = __floats2bfloat162_rn(v0, v1);
-    else {
-      D[0] = __float2bfloat16(v0);
-      if (two) D[1] = __float2bfloat16(v1);
     }
   }
 }
 
-// The bf16 pair (off, off + 1) of an epilogue input; the second element reads as 0 when it is past the last column.
-template <bool EDGE>
-__device__ __forceinline__ __nv_bfloat162 load_pair(const __nv_bfloat16* src, long long off, bool two, bool vec) {
-  if (!EDGE || vec) return __ldg(reinterpret_cast<const __nv_bfloat162*>(src + off));
-  return __halves2bfloat162(src[off], two ? src[off + 1] : __float2bfloat16(0.0f));
+// ---- staged epilogue
+// A consumer warpgroup writes one 64-row half of its accumulators to its own 64 x BN fp32 staging buffer in shared
+// memory, then walks the half row by row: each thread takes 8 consecutive columns of a row, so every global access is
+// a 16-byte vector and a row segment is contiguous across threads.  The per-element code is one rolled loop for interior
+// and edge tiles alike, instead of a fully unrolled copy per accumulator register.
+constexpr int STAGE_U = 2;   // rows per thread and loop iteration; the next iteration's global inputs are prefetched
+
+// Byte offset of the 16-byte chunk holding columns 4 c .. 4 c + 3 of staged row r.  XOR swizzle: the 8-byte fragment
+// stores of a half-warp (rows r0 .. r0 + 3, 8 columns) and the 16-byte row loads of a quarter-warp (8 threads of one
+// row, chunks 2 g or 2 g + 1) both touch 32 distinct banks.
+template <int BN>
+__device__ __forceinline__ uint32_t stage_off(int r, int c) {
+  return (uint32_t)(r * BN * 4 + ((c ^ (2 * (r & 3)) ^ ((c >> 3) & 1)) << 4));
 }
 
-// Epilogue of one 128 x BN tile straight from a warpgroup's accumulator registers: acc[hh] holds rows 64 hh .. 64 hh + 63
-// in the wgmma fragment order (thread rows r0, r0 + 8; columns 8 j + cq, + 1).  With only four warps per warpgroup
-// nothing hides a load's latency, so the loads of a group of JG column pairs (bias, aux_in, add_in for the thread's
-// four rows) are all issued before the group's first store.
-template <int BN, int EPI, bool EDGE>
-__device__ __forceinline__ void epilogue(const GemmKParams& p, const TileCoord& t, const float (&acc)[2][BN / 2], int r0,
-                                         int cq) {
-  constexpr int JG = 4;
-  const int n0 = t.n_tile * BN;
+__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+__device__ __forceinline__ float bf16_at(const uint4& v, int i) {
+  const uint32_t w = i < 2 ? v.x : i < 4 ? v.y : i < 6 ? v.z : v.w;
+  return (i & 1) ? bf16_hi(w) : bf16_lo(w);
+}
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return (uint32_t)__bfloat16_as_ushort(h.x) | ((uint32_t)__bfloat16_as_ushort(h.y) << 16);
+}
+
+// 8 bf16 at src + off, of which the first n (1 .. 8) exist; vec: all 8 exist and are 16-byte aligned.
+__device__ __forceinline__ uint4 load8(const __nv_bfloat16* src, long long off, int n, bool vec) {
+  if (vec) return __ldg(reinterpret_cast<const uint4*>(src + off));
+  uint32_t w[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t lo = 2 * k < n ? __bfloat16_as_ushort(src[off + 2 * k]) : 0u;
+    const uint32_t hi = 2 * k + 1 < n ? __bfloat16_as_ushort(src[off + 2 * k + 1]) : 0u;
+    w[k] = lo | (hi << 16);
+  }
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+__device__ __forceinline__ void store8_bf16(__nv_bfloat16* dst, long long off, int n, bool vec, const float (&v)[8]) {
+  if (vec) {
+    *reinterpret_cast<uint4*>(dst + off) =
+        make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i < n) dst[off + i] = __float2bfloat16(v[i]);
+  }
+}
+
+// The epilogue of 8 consecutive columns of one row at element offset `off`, of which the first n exist.  v: the
+// accumulators; b: bias (used when add_bias); mul_in / add_in: the aux_in and add_in values.  The per-element
+// arithmetic and its order are those of every earlier version of this kernel, so results are unchanged bit for bit.
+template <int EPI>
+__device__ __forceinline__ void epi_chunk(const GemmKParams& p, long long off, int n, bool vec, float (&v)[8],
+                                          const float (&b)[8], bool add_bias, const uint4& mul_in, const uint4& add_in) {
+  const bool generic = EPI == EPI_GENERIC;
+  const bool aux_out = generic ? p.aux_out != nullptr : EPI == EPI_GELU_PRE;
+  const int act = generic ? p.act : (EPI == EPI_GELU_PRE ? 1 : 0);
+  const int mul = epi_mul_of<EPI>(p);
+  const bool add = epi_add_of<EPI>(p);
+  const bool drop = (generic || EPI >= EPI_GELU_PRE) && p.drop_thresh != 0;
+  const bool out_f32 = (generic || EPI == EPI_PLAIN) && p.out_f32 != 0;
+  const bool fast_gelu = generic && p.fast_gelu;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    v[i] *= p.alpha;
+    if (add_bias) v[i] += b[i];
+  }
+  if (aux_out) store8_bf16(p.aux_out, off, n, vec, v);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (act == 1) v[i] = fast_gelu ? gelu_fast(v[i]) : gelu_erf(v[i]);
+    else if (act == 2) v[i] = fmaxf(v[i], 0.0f);
+    if (mul == 1) v[i] *= fast_gelu ? dgelu_fast(bf16_at(mul_in, i)) : dgelu_erf(bf16_at(mul_in, i));
+    else if (mul == 2) v[i] = bf16_at(mul_in, i) > 0.0f ? v[i] : 0.0f;
+    if (drop) v[i] = drop_keep(p.drop_seed, (uint64_t)(off + i), p.drop_thresh) ? v[i] * p.drop_scale : 0.0f;
+    if (add) v[i] += bf16_at(add_in, i);
+  }
+  if (out_f32) {
+    float* D = reinterpret_cast<float*>(p.D) + off;
+    if (vec) {
+      reinterpret_cast<float4*>(D)[0] = make_float4(v[0], v[1], v[2], v[3]);
+      reinterpret_cast<float4*>(D)[1] = make_float4(v[4], v[5], v[6], v[7]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (i < n) D[i] = v[i];
+    }
+  } else {
+    store8_bf16(reinterpret_cast<__nv_bfloat16*>(p.D), off, n, vec, v);
+  }
+}
+
+// Staged epilogue of one 128 x BN tile (see above).  stage_buf: this warpgroup's 64 x BN fp32 buffer; barrier 3 + c
+// spans the warpgroup only.  Thread tid owns columns 8 g .. 8 g + 7 (g = tid % (BN / 8)) of rows rs, rs + RP, ...
+template <int BN, int EPI>
+__device__ __forceinline__ void epilogue_staged(const GemmKParams& p, const TileCoord& t, const float (&acc)[2][BN / 2],
+                                                uint8_t* stage_buf, int r0, int cq, int c) {
+  constexpr int TPR = BN / 8;                     // threads per row
+  constexpr int RP = CONSUMER_THREADS / TPR;      // rows per pass of the warpgroup
+  constexpr int GROUPS = 64 / (RP * STAGE_U);     // loop iterations per half
+  // Prefetch the next iteration's aux_in / add_in; GENERIC (two inputs) loads them in the iteration instead, so that
+  // it needs no spills.
+  constexpr bool PREFETCH = EPI != EPI_GENERIC;
+  const int tid = threadIdx.x % CONSUMER_THREADS;
+  const int g = tid % TPR, rs = tid / TPR;
+  const int col = t.n_tile * BN + 8 * g;
+  const int n = min(8, p.N - col);                // columns of the thread's chunk that exist (<= 0: none)
+  const bool vec = p.vec_ok && n == 8;
   const bool add_bias = p.bias != nullptr && t.split == 0;
   const bool mul = epi_mul_of<EPI>(p) != 0;
   const bool add = epi_add_of<EPI>(p);
-  const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2;
-  long long row_off[4];
-  bool row_ok[4];
+  float b[8];
 #pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const int row = t.m_tile * BLOCK_M + 64 * (r >> 1) + r0 + 8 * (r & 1);
-    row_ok[r] = !EDGE || row < p.M;
-    row_off[r] = batch_off + (long long)row * p.ldd;
-  }
+  for (int i = 0; i < 8; ++i) b[i] = add_bias && i < n ? __ldg(p.bias + col + i) : 0.0f;
+  const long long batch_off = (long long)t.b1 * p.d_s1 + (long long)t.b2 * p.d_s2 + col;
+  const uint32_t sbuf = smem_u32(stage_buf);
+  const int row0 = t.m_tile * BLOCK_M + rs;
+
+  // global inputs of the STAGE_U rows of loop iteration k of half hh
+  auto load_inputs = [&](int hh, int k, uint4 (&mi)[STAGE_U], uint4 (&ai)[STAGE_U]) {
 #pragma unroll
-  for (int j0 = 0; j0 < BN / 8; j0 += JG) {
-    float b[JG][2];
-    __nv_bfloat162 mul_in[JG][4], add_v[JG][4];
-#pragma unroll
-    for (int jj = 0; jj < JG; ++jj) {
-      const int col = n0 + 8 * (j0 + jj) + cq;
-      const bool col_ok = !EDGE || col < p.N;
-      const bool two = !EDGE || col + 1 < p.N;
-      const bool vec = !EDGE || (two && p.vec_ok);
-      b[jj][0] = add_bias && col_ok ? __ldg(p.bias + col) : 0.0f;
-      b[jj][1] = add_bias && col_ok && two ? __ldg(p.bias + col + 1) : 0.0f;
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const bool ok = col_ok && row_ok[r];
-        mul_in[jj][r] = mul && ok ? load_pair<EDGE>(p.aux_in, row_off[r] + col, two, vec) : __nv_bfloat162();
-        add_v[jj][r] = add && ok ? load_pair<EDGE>(p.add_in, row_off[r] + col, two, vec) : __nv_bfloat162();
-      }
+    for (int u = 0; u < STAGE_U; ++u) {
+      const int row = row0 + 64 * hh + (k * STAGE_U + u) * RP;
+      const bool ok = n > 0 && row < p.M;
+      const long long off = batch_off + (long long)row * p.ldd;
+      mi[u] = mul && ok ? load8(p.aux_in, off, n, vec) : make_uint4(0, 0, 0, 0);
+      ai[u] = add && ok ? load8(p.add_in, off, n, vec) : make_uint4(0, 0, 0, 0);
     }
+  };
+
+#pragma unroll 1
+  for (int hh = 0; hh < 2; ++hh) {
+    uint4 mi[STAGE_U], ai[STAGE_U];
+    if (PREFETCH) load_inputs(hh, 0, mi, ai);
+    // phase 1: fragments -> staging buffer, once every thread has read the previous half out of it
+    named_bar_sync(3 + c, CONSUMER_THREADS);
+    if (hh == 0) {
 #pragma unroll
-    for (int jj = 0; jj < JG; ++jj) {
-      const int j = j0 + jj;
-      const int col = n0 + 8 * j + cq;
-      if (EDGE && col >= p.N) continue;
+      for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int hh = r >> 1, h = r & 1;
-        if (row_ok[r])
-          epi_pair<EPI, EDGE>(p, row_off[r] + col, col, acc[hh][4 * j + 2 * h], acc[hh][4 * j + 2 * h + 1], add_bias,
-                              b[jj][0], b[jj][1], mul_in[jj][r], add_v[jj][r]);
+        for (int h = 0; h < 2; ++h)
+          st_shared_v2(sbuf + stage_off<BN>(r0 + 8 * h, 2 * j + (cq >> 2)) + (cq & 2) * 4, acc[0][4 * j + 2 * h],
+                       acc[0][4 * j + 2 * h + 1]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          st_shared_v2(sbuf + stage_off<BN>(r0 + 8 * h, 2 * j + (cq >> 2)) + (cq & 2) * 4, acc[1][4 * j + 2 * h],
+                       acc[1][4 * j + 2 * h + 1]);
+    }
+    named_bar_sync(3 + c, CONSUMER_THREADS);
+    // phase 2: rows of the staged half, STAGE_U per iteration, the next iteration's inputs in flight
+#pragma unroll 1
+    for (int k = 0; k < GROUPS; ++k) {
+      uint4 mi_next[STAGE_U] = {}, ai_next[STAGE_U] = {};
+      if (!PREFETCH) load_inputs(hh, k, mi, ai);
+      else if (k + 1 < GROUPS) load_inputs(hh, k + 1, mi_next, ai_next);
+      float v[STAGE_U][8];
+#pragma unroll
+      for (int u = 0; u < STAGE_U; ++u) {
+        const int rl = rs + (k * STAGE_U + u) * RP;
+        const float4 x = ld_shared_v4f(sbuf + stage_off<BN>(rl, 2 * g));
+        const float4 y = ld_shared_v4f(sbuf + stage_off<BN>(rl, 2 * g + 1));
+        v[u][0] = x.x; v[u][1] = x.y; v[u][2] = x.z; v[u][3] = x.w;
+        v[u][4] = y.x; v[u][5] = y.y; v[u][6] = y.z; v[u][7] = y.w;
+      }
+#pragma unroll
+      for (int u = 0; u < STAGE_U; ++u) {
+        const int row = row0 + 64 * hh + (k * STAGE_U + u) * RP;
+        if (n > 0 && row < p.M)
+          epi_chunk<EPI>(p, batch_off + (long long)row * p.ldd, n, vec, v[u], b, add_bias, mi[u], ai[u]);
+      }
+      if (PREFETCH) {
+#pragma unroll
+        for (int u = 0; u < STAGE_U; ++u) {
+          mi[u] = mi_next[u];
+          ai[u] = ai_next[u];
+        }
       }
     }
   }
@@ -382,8 +469,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmKParams p, int total_tiles) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment for SWIZZLE_128B atoms
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte alignment for SWIZZLE_128B atoms.  Layout: [staging buffers of the two consumer warpgroups, staged
+  // variants only] [stage ring] [barriers]
+  uint8_t* stage_bufs = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = stage_bufs + staging_bytes(BN, EPI);
   constexpr int B_STAGE_BYTES = BN * BLOCK_K * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * STAGE_BYTES);
@@ -486,13 +575,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 2] = gtimer();
       }
       const bool interior = p.vec_ok && (t.m_tile + 1) * BLOCK_M <= p.M && (t.n_tile + 1) * BN <= p.N;
-      if constexpr (EPI == EPI_SPLIT_DET) {
+      if constexpr (epi_staged(EPI)) {
+        epilogue_staged<BN, EPI>(p, t, acc, stage_bufs + c * (staging_bytes(BN, EPI) / 2), r0, cq, c);
+      } else if constexpr (EPI == EPI_SPLIT_DET) {
         int* ticket = reinterpret_cast<int*>(empty_bar + MAX_STAGES) + c;
         if (interior) epilogue_split_det<BN, false>(p, t, acc, r0, cq, c, ticket);
         else epilogue_split_det<BN, true>(p, t, acc, r0, cq, c, ticket);
       } else {
-        if (interior) epilogue<BN, EPI, false>(p, t, acc, r0, cq);
-        else epilogue<BN, EPI, true>(p, t, acc, r0, cq);
+        if (interior) epilogue_atomic<BN, false>(p, t, acc, r0, cq);
+        else epilogue_atomic<BN, true>(p, t, acc, r0, cq);
       }
       if (stamp) p.trace[((long long)blockIdx.x * 16 + lt) * 4 + 3] = gtimer();
     }
@@ -740,7 +831,8 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   }
 
   const int stage_bytes = A_STAGE_BYTES + bn * BLOCK_K * 2;
-  int stages = (g_smem_optin - 1024 - 256) / stage_bytes;
+  const int staging = staging_bytes(bn, epi);
+  int stages = (g_smem_optin - 1024 - 256 - staging) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   {
     static int env_stages = -1;  // BB_GEMM_STAGES: pipeline-depth experiments only
@@ -752,7 +844,7 @@ extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   }
   if (stages < 2) return set_error("bb_gemm_bf16: not enough shared memory for 2 stages");
   p.stages = stages;
-  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + 256;
+  const size_t smem_bytes = (size_t)staging + (size_t)stages * stage_bytes + 1024 + 256;
 
   CUtensorMap ta, tb;
   int e;

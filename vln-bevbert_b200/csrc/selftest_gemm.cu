@@ -66,6 +66,14 @@ __global__ void ref_gemm(const __nv_bfloat16* A, const __nv_bfloat16* B, float* 
 
 static float frand() { return (float)rand() / RAND_MAX * 2.f - 1.f; }
 
+// FNV-1a over raw output bytes: two builds of the library computed the same bits iff the hashes agree
+static unsigned long long fnv1a(const void* data, size_t n) {
+  const unsigned char* b = static_cast<const unsigned char*>(data);
+  unsigned long long h = 0xcbf29ce484222325ull;
+  for (size_t i = 0; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+  return h;
+}
+
 static int run_case(const Case& c) {
   const int nb = c.nb1 * c.nb2;
   // buffer extents (elements)
@@ -137,15 +145,19 @@ static int run_case(const Case& c) {
   std::vector<float> hRef(d_ext), hPre(d_ext), hOut(d_ext);
   CK(cudaMemcpy(hRef.data(), dRef, d_ext * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(hPre.data(), dPre, d_ext * 4, cudaMemcpyDeviceToHost));
+  unsigned long long hash_d;
   if (c.out_f32) {
     CK(cudaMemcpy(hOut.data(), dD, d_ext * 4, cudaMemcpyDeviceToHost));
+    hash_d = fnv1a(hOut.data(), d_ext * 4);
   } else {
     std::vector<__nv_bfloat16> t(d_ext);
     CK(cudaMemcpy(t.data(), dD, d_ext * 2, cudaMemcpyDeviceToHost));
     for (long long i = 0; i < d_ext; ++i) hOut[i] = __bfloat162float(t[i]);
+    hash_d = fnv1a(t.data(), d_ext * 2);
   }
   std::vector<__nv_bfloat16> hAuxOut(d_ext);
   CK(cudaMemcpy(hAuxOut.data(), dAuxOut, d_ext * 2, cudaMemcpyDeviceToHost));
+  const unsigned long long hash_aux = fnv1a(hAuxOut.data(), d_ext * 2);
   double max_err = 0, max_ref = 0, max_aux_err = 0;
   long long bad_i = -1;
   // compare only addressed outputs; everything else must still be zero (catches stray writes)
@@ -207,8 +219,9 @@ static int run_case(const Case& c) {
     cudaFree(dT);
   }
   double tflops = ms > 0 ? 2.0 * c.M * c.N * c.K * nb / (ms * 1e-3) / 1e12 : 0;
-  printf("CASE %-22s %s max_err=%.4g (at %lld) max_ref=%.4g aux_err=%.4g stray=%lld  %.3f ms %.1f TFLOP/s\n", c.name,
-         ok ? "PASS" : "FAIL", max_err, bad_i, max_ref, max_aux_err, stray, ms, tflops);
+  printf("CASE %-22s %s max_err=%.4g (at %lld) max_ref=%.4g aux_err=%.4g stray=%lld  %.3f ms %.1f TFLOP/s  "
+         "hash D=%016llx aux=%016llx\n", c.name, ok ? "PASS" : "FAIL", max_err, bad_i, max_ref, max_aux_err, stray, ms,
+         tflops, hash_d, hash_aux);
   if (!ok && bad_i >= 0) {
     // print a small window of outputs around the first row for diagnosis
     printf("   first 8 outputs: ");
