@@ -19,7 +19,9 @@ from bevbert_b200.optim import AdamW, build_param_groups  # noqa: E402
 from bevbert_b200.parallel import direct_param_grads, enable_side_stream  # noqa: E402
 
 
-def main():
+def make_cycle():
+    """Builds bench.py's flagship model, optimiser and one batch per task of its mix; returns a function that runs one
+    task cycle (every task of the mix once: forward, backward, optimiser step) and synchronises."""
     torch.manual_seed(0)
     model = synth.det_init_(GlocalTextPathCMTPreTraining(bench.full_config()), seed=3).cuda().train()
     direct_param_grads(True)
@@ -36,7 +38,12 @@ def main():
             opt.step()
             opt.zero_grad(set_to_none=True)
         torch.cuda.synchronize()
+    return cycle
 
+
+def main():
+    cycle = make_cycle()
+    mix = bench.MIX
     per = {}
     for det in (False, True):
         torch.use_deterministic_algorithms(det)

@@ -6,7 +6,10 @@
 //   attn_tc_fwd_kernel     forward: a CTA owns 128 queries of one (sample, head); K / V stream through a ring of
 //                          shared-memory stages in 64-key blocks;
 //   attn_tc_bwd_kernel<M>  backward, dQ pass (M = 0, CTA = 128 queries) and dK / dV pass (M = 1, CTA = 128 keys).
-// Every CTA is two consumer warpgroups (warps 0..7, 64 rows each) and one TMA producer warp (warp 8).  Scores are
+// Every CTA is two consumer warpgroups (warps 0..7, 64 rows each) and one TMA producer warp (warp 8; in the backward
+// a whole producer warpgroup, for setmaxnreg), which also writes the streamed block's per-column state into the
+// stage next to the tiles (the key mask; in the dK / dV pass -lse, D and the dropout row hash of each query), so the
+// consumers read it from shared memory once per block instead of every thread loading or hashing it.  Scores are
 // wgmma accumulators in registers: thread t of a warpgroup holds rows r0 = 16 (t / 32) + (t % 32) / 4 and r0 + 8 and,
 // of every 8-column group, columns 2 (t % 4) and 2 (t % 4) + 1, so a row lives in the four threads of a quad and row
 // reductions are two shuffles.  That fragment, converted to bf16, is exactly the register A operand of the next
@@ -35,7 +38,9 @@ namespace fat {
 typedef __nv_bfloat16 bf16;
 constexpr int BM = 128;          // rows per CTA (two warpgroups of 64)
 constexpr int KB = 64;           // keys (forward, MODE 0) or queries (MODE 1) per streamed block
-constexpr int NT = 288;          // 8 consumer warps + 1 producer warp
+constexpr int NT = 288;          // forward: 8 consumer warps + 1 producer warp
+constexpr int NT_BWD = 384;      // backward: 2 consumer warpgroups + 1 producer warpgroup (setmaxnreg needs whole ones)
+constexpr int BWD_PRODUCER_REGS = 40, BWD_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers per SM
 constexpr int NST = 3;           // depth of the streamed-block ring
 constexpr int R_BYTES = BM * 128, BLK_BYTES = KB * 128;
 constexpr float LOG2E = 1.4426950408889634f;
@@ -104,9 +109,16 @@ __device__ __forceinline__ void pv_product(float (&d)[32], const uint32_t (&a)[4
 __device__ __forceinline__ void store_row_pair(bf16* dst, float v0, float v1) {
   *reinterpret_cast<uint32_t*>(dst) = pack2(v0, v1);
 }
+// log2-domain key mask of key k (-inf past the last key)
+__device__ __forceinline__ float key_mask_l2(const float* kmask, int b, int nk, int k) {
+  return k < nk ? (kmask ? __ldg(kmask + (int64_t)b * nk + k) * LOG2E : 0.f) : -INFINITY;
+}
 
 // ================================================================================================ forward
-__global__ void __launch_bounds__(NT, 1)
+// 2 CTAs per SM (<= 112 registers): while one CTA's warpgroups run their softmax, the other's MMAs keep the tensor
+// pipe busy.  The per-key mask is staged by the producer warp into the ring next to K / V instead of being held in
+// registers.
+__global__ void __launch_bounds__(NT, 2)
 attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                    const __grid_constant__ CUtensorMap tv, const FwdParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -114,7 +126,8 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + R_BYTES;
   uint8_t* sV = sK + NST * BLK_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + NST * BLK_BYTES);
+  float* sM = reinterpret_cast<float*>(sV + NST * BLK_BYTES);   // [NST][KB] log2-domain key mask of the block
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sM + NST * KB);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;          // [NST]
   uint64_t* kv_free = bars + 1 + NST;    // [NST]
@@ -139,13 +152,17 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   pdl_trigger();
 
   if (warp == 8) {
-    // ------------------------------------------------------------------ TMA producer
+    // ------------------------------------------------------------------ TMA producer (+ key mask of the block)
     if (lane == 0) {
       mbar_expect_tx(q_full, R_BYTES);
       tma_load_4d(sQ, &tq, q_full, 0, q0, h, b);
-      for (int j = 0; j < nblk; ++j) {
-        const int st = j % NST;
-        mbar_wait_relaxed(&kv_free[st], ((j / NST) & 1) ^ 1);
+    }
+    for (int j = 0; j < nblk; ++j) {
+      const int st = j % NST;
+      mbar_wait_relaxed(&kv_free[st], ((j / NST) & 1) ^ 1);
+      for (int c = lane; c < KB; c += 32) sM[st * KB + c] = key_mask_l2(p.kmask, b, p.nk, j * KB + c);
+      __syncwarp();   // the mask stores precede lane 0's arrive, which publishes them with the stage
+      if (lane == 0) {
         mbar_expect_tx(&kv_full[st], 2 * BLK_BYTES);
         tma_load_4d(sK + st * BLK_BYTES, &tk, &kv_full[st], 0, j * KB, h, b);
         tma_load_4d(sV + st * BLK_BYTES, &tv, &kv_full[st], 0, j * KB, h, b);
@@ -173,14 +190,6 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   mbar_wait(q_full, 0);
   for (int j = 0; j < nblk; ++j) {
     const int st = j % NST;
-    float km[16];   // log2-domain key mask of this thread's 16 columns
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int c = j * KB + 8 * jj + cq + e;
-        km[2 * jj + e] = c < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + c) * LOG2E : 0.f) : -INFINITY;
-      }
     mbar_wait(&kv_full[st], (j / NST) & 1);
     float s[32];
     fence_regs(s);
@@ -191,13 +200,15 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
     fence_regs(s);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 km = *reinterpret_cast<const float2*>(sM + st * KB + 8 * jj + cq);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         float& v = s[4 * jj + i];
-        v = fmaf(v, p.a2, km[2 * jj + (i & 1)]);
+        v = fmaf(v, p.a2, (i & 1) ? km.y : km.x);
         mx[i >> 1] = fmaxf(mx[i >> 1], v);
       }
+    }
     float ms[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
@@ -277,8 +288,11 @@ struct BwdParams {
 
 // tr0 / tr1: the CTA's resident 128-row tiles (Q, dO for MODE 0; K, V for MODE 1), box 128 rows;
 // ts0 / ts1: the streamed 64-row blocks (K, V for MODE 0; Q, dO for MODE 1), box 64 rows.
+// The producer is a whole warpgroup (warps 8..11, only warp 8 works) so that setmaxnreg can move registers from it to
+// the consumers: a 288-thread CTA is held to 168 registers per thread, at which the dK / dV pass's staged per-query
+// state spills.
 template <int MODE>
-__global__ void __launch_bounds__(NT, 1)
+__global__ void __launch_bounds__(NT_BWD, 1)
 attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constant__ CUtensorMap tr1,
                    const __grid_constant__ CUtensorMap ts0, const __grid_constant__ CUtensorMap ts1, const BwdParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -287,7 +301,10 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constan
   uint8_t* sR1 = sR0 + R_BYTES;
   uint8_t* sS0 = sR1 + R_BYTES;             // [NST] streamed block 0 (K_j / Q_i)
   uint8_t* sS1 = sS0 + NST * BLK_BYTES;     // [NST] streamed block 1 (V_j / dO_i)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sS1 + NST * BLK_BYTES);
+  // [NST][3][KB] per-column state of the streamed block, written by the producer warp with the stage:
+  // MODE 0 -> log2-domain key mask; MODE 1 -> -lse, D and the dropout row hash of the query
+  float* sC = reinterpret_cast<float*>(sS1 + NST * BLK_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sC + NST * 3 * KB);
   uint64_t* r_full = bars;
   uint64_t* st_full = bars + 1;          // [NST]
   uint64_t* st_free = bars + 1 + NST;    // [NST]
@@ -312,14 +329,32 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constan
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 8) {
+  const int64_t bh = (int64_t)b * p.H + h;
+  if (warp >= 8) {
+    setmaxnreg_dec<BWD_PRODUCER_REGS>();
+    if (warp > 8) return;
     if (lane == 0) {
       mbar_expect_tx(r_full, 2 * R_BYTES);
       tma_load_4d(sR0, &tr0, r_full, 0, t0, h, b);
       tma_load_4d(sR1, &tr1, r_full, 0, t0, h, b);
-      for (int j = 0; j < nblk; ++j) {
-        const int st = j % NST;
-        mbar_wait_relaxed(&st_free[st], ((j / NST) & 1) ^ 1);
+    }
+    for (int j = 0; j < nblk; ++j) {
+      const int st = j % NST;
+      mbar_wait_relaxed(&st_free[st], ((j / NST) & 1) ^ 1);
+      float* cs = sC + st * 3 * KB;
+      for (int c = lane; c < KB; c += 32) {
+        const int col = j * KB + c;
+        if (MODE == 0) {
+          cs[c] = key_mask_l2(p.kmask, b, p.nk, col);
+        } else {
+          const bool ok = col < p.nq;
+          cs[c] = ok ? -__ldg(p.lse + bh * p.nq + col) : -INFINITY;
+          cs[KB + c] = ok ? __ldg(p.dsum + bh * p.nq + col) : 0.f;
+          cs[2 * KB + c] = __uint_as_float(p.thresh ? rng_u32(p.seed, (uint64_t)(bh * p.nq + col)) : 0u);
+        }
+      }
+      __syncwarp();   // the state stores precede lane 0's arrive, which publishes them with the stage
+      if (lane == 0) {
         mbar_expect_tx(&st_full[st], 2 * BLK_BYTES);
         tma_load_4d(sS0 + st * BLK_BYTES, &ts0, &st_full[st], 0, j * KB, h, b);
         tma_load_4d(sS1 + st * BLK_BYTES, &ts1, &st_full[st], 0, j * KB, h, b);
@@ -328,12 +363,12 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constan
     return;
   }
 
+  setmaxnreg_inc<BWD_CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int r0 = (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   const uint32_t t16s = p.thresh & 0xFFFF0000u;
   const float scale_eff = p.thresh ? p.scale : 1.0f, inv_scale = 1.0f / scale_eff, as_ = p.alpha * scale_eff;
-  const int64_t bh = (int64_t)b * p.H + h;
   const uint32_t aR0 = smem_u32(sR0) + wg * 8192, aR1 = smem_u32(sR1) + wg * 8192;
   int row[2];   // this thread's two rows: queries (MODE 0) / keys (MODE 1)
 #pragma unroll
@@ -402,18 +437,18 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constan
     for (int jj = 0; jj < 8; ++jj) {
       const int c = j * KB + 8 * jj + cq;
       // per-column state: MODE 0 -> key mask; MODE 1 -> -lse, D / scale and the dropout hash of the query
-      float ca[2], cb[2] = {0.f, 0.f};
+      const float* cs = sC + st * 3 * KB + 8 * jj + cq;
+      const float2 ca2 = *reinterpret_cast<const float2*>(cs);
+      const float ca[2] = {ca2.x, ca2.y};
+      float cb[2] = {0.f, 0.f};
       uint32_t ch[2] = {0u, 0u};
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        if (MODE == 0) {
-          ca[e] = c + e < p.nk ? (p.kmask ? __ldg(p.kmask + (int64_t)b * p.nk + c + e) * LOG2E : 0.f) : -INFINITY;
-        } else {
-          const bool ok = c + e < p.nq;
-          ca[e] = ok ? -__ldg(p.lse + bh * p.nq + c + e) : -INFINITY;
-          cb[e] = ok ? __ldg(p.dsum + bh * p.nq + c + e) * inv_scale : 0.f;
-          ch[e] = p.thresh ? rng_u32(p.seed, (uint64_t)(bh * p.nq + c + e)) : 0u;
-        }
+      if (MODE == 1) {
+        const float2 cb2 = *reinterpret_cast<const float2*>(cs + KB);
+        const float2 ch2 = *reinterpret_cast<const float2*>(cs + 2 * KB);
+        cb[0] = cb2.x * inv_scale;   // D is 0 past the last query, and 0 * inv_scale = 0
+        cb[1] = cb2.y * inv_scale;
+        ch[0] = __float_as_uint(ch2.x);
+        ch[1] = __float_as_uint(ch2.y);
       }
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
@@ -492,8 +527,8 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tr0, const __grid_constan
   }
 }
 
-constexpr size_t FWD_SMEM = 1024 + R_BYTES + 2 * (size_t)NST * BLK_BYTES + (1 + 2 * NST) * 8;
-constexpr size_t BWD_SMEM = 1024 + 2 * R_BYTES + 2 * (size_t)NST * BLK_BYTES + (1 + 2 * NST) * 8;
+constexpr size_t FWD_SMEM = 1024 + R_BYTES + 2 * (size_t)NST * BLK_BYTES + NST * KB * 4 + (1 + 2 * NST) * 8;
+constexpr size_t BWD_SMEM = 1024 + 2 * R_BYTES + 2 * (size_t)NST * BLK_BYTES + NST * 3 * KB * 4 + (1 + 2 * NST) * 8;
 
 static int g_init = 0;
 static int init_once() {
@@ -584,8 +619,8 @@ int launch_bwd(const bb_flash_args* a, void* stream) {
   if (int e = make_tmap_bf16_4d(&tv64, a->v, 64, a->nk, a->H, a->B, a->ldv, 64, a->v_bs, KB)) return e;
   const dim3 gq((unsigned)((a->nq + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
   const dim3 gk((unsigned)((a->nk + BM - 1) / BM), (unsigned)a->H, (unsigned)a->B);
-  launch_pdl(attn_tc_bwd_kernel<0>, gq, dim3(NT), BWD_SMEM, (cudaStream_t)stream, tq, tdo, tk64, tv64, p);
-  launch_pdl(attn_tc_bwd_kernel<1>, gk, dim3(NT), BWD_SMEM, (cudaStream_t)stream, tk, tv, tq64, tdo64, p);
+  launch_pdl(attn_tc_bwd_kernel<0>, gq, dim3(NT_BWD), BWD_SMEM, (cudaStream_t)stream, tq, tdo, tk64, tv64, p);
+  launch_pdl(attn_tc_bwd_kernel<1>, gk, dim3(NT_BWD), BWD_SMEM, (cudaStream_t)stream, tk, tv, tq64, tdo64, p);
   count_launch(2);
   return check_launch("attn_tc_bwd kernels");
 }
