@@ -266,7 +266,8 @@ int bb_attn_scores(const bb_attn_scores_args* args, void* stream);
  * B x H independent (sample, head) problems without materialising scores or probabilities in HBM
  * (vilmodel.py:103-154 BertSelfAttention, 325-363 BertOutAttention; transformer.py:170-182 panorama encoder).
  * Element (b, row, h, d) of q / k / v / o / dout / dq / dk / dv is at  ptr + b*X_bs + row*ldX + h*64 + d  (bf16), so
- * per-head views into packed Q|K|V buffers need no copies.  kmask (B,nk) and bias (B,nq,nk) are additive fp32
+ * per-head views into packed Q|K|V buffers need no copies.  q / k / v / o / dout / dq / dk / dv must be 16-byte aligned
+ * and every row stride ld* and batch stride *_bs a multiple of 8 elements; other calls are rejected.  kmask (B,nk) and bias (B,nq,nk) are additive fp32
  * (may be NULL); lse (B,H,nq) receives the row log-sum-exp (log2 domain) and is the only tensor saved for backward
  * besides o; rows whose keys are all -inf give zeros.  Dropout: element (b,h,q,k) is kept iff a 16-bit half of
  * mix(hash(seed, (b*H+h)*nq+q), k/2) is >= thresh >> 16 (one row hash, one mix per pair of adjacent keys); kept

@@ -114,11 +114,62 @@ def _flash_probs(q, k, B, H, nq, nk, ldq, ldk, kmask, bias):
     return torch.nan_to_num(torch.softmax(s, -1), nan=0.0)          # rows with every key at -inf give zeros
 
 
+_LOG2E = torch.tensor(1.4426950408889634, dtype=F32)
+
+
+def _flash_logits2(qh, kh, alpha, kmask, bias):
+    """log2-domain logits in the kernels' fp32 order: fma(S, alpha log2e, kmask log2e) (+ bias log2e); (B,H,nq,nk)"""
+    B, H, nq, nk = qh.shape[0], qh.shape[1], qh.shape[2], kh.shape[2]
+    a2 = (torch.tensor(alpha, dtype=F32) * _LOG2E).double()
+    s = torch.matmul(qh.to(F32), kh.to(F32).transpose(-1, -2)).double() * a2
+    if kmask is not None:
+        s = s + (kmask.to(F32) * _LOG2E).double().view(B, 1, 1, nk)
+    s = s.to(F32).double()
+    if bias is not None:
+        s = s + bias.to(F32).double().view(B, 1, nq, nk) * _LOG2E.double()
+    return s.to(F32)
+
+
+def flash_core_fwd(q, k, v, o, lse, alpha, kmask=None, bias=None):
+    """bb_flash_fwd restated in fp32 on (B, rows, H, 64) views (any strides): ex2 of the log2-domain logits against the
+    row maximum, bf16 probabilities into the P V product, one scale by 1/l, LSE = max + log2 l (+inf for rows whose
+    keys are all -inf, which give zeros).  Dropout is not emulated."""
+    qh, kh, vh = (t.permute(0, 2, 1, 3) for t in (q, k, v))
+    s = _flash_logits2(qh, kh, alpha, kmask, bias)
+    m = s.amax(-1, keepdim=True)
+    e = torch.exp2(s - torch.where(m == float("-inf"), torch.zeros_like(m), m))
+    l = e.sum(-1, keepdim=True)
+    oh = torch.matmul(e.to(torch.bfloat16).to(F32), vh.to(F32)) * torch.where(l > 0, 1.0 / l, torch.zeros_like(l))
+    o.copy_(oh.permute(0, 2, 1, 3).to(o.dtype))
+    lse.copy_(torch.where(l > 0, m + torch.log2(l), torch.full_like(l, float("inf")))[..., 0])
+
+
+def flash_core_bwd(q, k, v, o, lse, dout, dq, dk, dv, alpha, kmask=None, bias=None, dbias=None):
+    """bb_flash_bwd restated in fp32 on (B, rows, H, 64) views: P = ex2(logit - lse), D = rowsum(dO o O),
+    dS = P (dO V^T - D) (dbias += sum over heads), dQ = bf16(alpha dS) K, dK = bf16(alpha dS)^T Q, dV = bf16(P)^T dO."""
+    qh, kh, vh, oh, doh = (t.permute(0, 2, 1, 3).to(F32) for t in (q, k, v, o, dout))
+    s = _flash_logits2(qh, kh, alpha, kmask, bias)
+    p = torch.exp2(s - lse.unsqueeze(-1))
+    d = (doh * oh).sum(-1, keepdim=True)
+    ds = p * (torch.matmul(doh, vh.transpose(-1, -2)) - d)
+    if dbias is not None:
+        dbias.add_(ds.sum(1))
+    dsb = (ds * alpha).to(torch.bfloat16).to(F32)
+    dq.copy_(torch.matmul(dsb, kh).permute(0, 2, 1, 3).to(dq.dtype))
+    dk.copy_(torch.matmul(dsb.transpose(-1, -2), qh).permute(0, 2, 1, 3).to(dk.dtype))
+    dv.copy_(torch.matmul(p.to(torch.bfloat16).to(F32).transpose(-1, -2), doh).permute(0, 2, 1, 3).to(dv.dtype))
+
+
 def flash_fwd(q, k, v, B, H, nq, nk, ldq, ldk, ldv, kmask=None, bias=None, drop=(0, 0, 1.0)):
     assert drop[1] == 0, "emulation runs with dropout disabled"
     p = _flash_probs(q, k, B, H, nq, nk, ldq, ldk, kmask, bias)
     o = torch.matmul(_a(p, 'flash_p').to(F32), _heads(v, B, nk, H, ldv).to(F32))          # (B,H,nq,64); P feeds the MMA as ACT
-    return _a(o.permute(0, 2, 1, 3).reshape(B, nq, H * 64).contiguous(), 'flash_o'), torch.zeros(B, H, nq, dtype=F32)
+    qh, kh = _heads(q, B, nq, H, ldq).to(F32), _heads(k, B, nk, H, ldk).to(F32)
+    s = _flash_logits2(qh, kh, 0.125, kmask, bias)                                        # the row log-sum-exp, log2 domain
+    m = s.amax(-1, keepdim=True)
+    l = torch.exp2(s - torch.where(m == float("-inf"), torch.zeros_like(m), m)).sum(-1, keepdim=True)
+    lse = torch.where(l > 0, m + torch.log2(l), torch.full_like(l, float("inf")))[..., 0]
+    return _a(o.permute(0, 2, 1, 3).reshape(B, nq, H * 64).contiguous(), 'flash_o'), lse
 
 
 def flash_bwd(q, k, v, o, lse, dout, B, H, nq, nk, ldq, ldk, ldv, kmask=None, bias=None, drop=(0, 0, 1.0), dbias=None,

@@ -593,9 +593,19 @@ static int fill(Params& p, const bb_flash_args* a, bool bwd) {
   p.B = a->B; p.H = a->H; p.nq = a->nq; p.nk = a->nk; p.alpha = a->alpha;
   p.seed = a->seed; p.thresh = a->thresh; p.scale = a->scale;
   if (!a->o || !a->lse) return set_error("bb_flash: null o / lse");
+  // both cores move 16-byte chunks of every row of every sample (cp.async / uint4 here, TMA in attn_tc.cu)
+  if ((reinterpret_cast<uintptr_t>(a->q) | reinterpret_cast<uintptr_t>(a->k) | reinterpret_cast<uintptr_t>(a->v) |
+       reinterpret_cast<uintptr_t>(a->o)) & 15)
+    return set_error("bb_flash: q / k / v / o must be 16-byte aligned");
+  if ((a->q_bs | a->k_bs | a->v_bs | a->o_bs) % 8) return set_error("bb_flash: batch strides must be multiples of 8 elements");
   if (bwd) {
     if (!a->dout || !a->dq || !a->dk || !a->dv || !a->dsum) return set_error("bb_flash_bwd: null gradient pointer");
     if ((a->lddo | a->lddq | a->lddk | a->lddv) % 8) return set_error("bb_flash_bwd: row strides must be multiples of 8");
+    if ((reinterpret_cast<uintptr_t>(a->dout) | reinterpret_cast<uintptr_t>(a->dq) | reinterpret_cast<uintptr_t>(a->dk) |
+         reinterpret_cast<uintptr_t>(a->dv)) & 15)
+      return set_error("bb_flash_bwd: dout / dq / dk / dv must be 16-byte aligned");
+    if ((a->do_bs | a->dq_bs | a->dk_bs | a->dv_bs) % 8)
+      return set_error("bb_flash_bwd: batch strides must be multiples of 8 elements");
     p.dout = (const bf16*)a->dout; p.do_bs = a->do_bs; p.lddo = a->lddo; p.dsum = a->dsum;
     p.dq = (bf16*)a->dq; p.dq_bs = a->dq_bs; p.lddq = a->lddq;
     p.dk = (bf16*)a->dk; p.dk_bs = a->dk_bs; p.lddk = a->lddk;
