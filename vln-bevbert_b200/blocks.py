@@ -167,10 +167,16 @@ class WeightCache:
         """Every shadow is out of date (parameters changed behind the cache's back)."""
         self.epoch += 1
 
-    def refresh_all(self):
+    def refresh_all(self, padded=False):
         """Advance the epoch and re-cast every plain / stacked bf16 shadow in ONE multi-tensor launch; padded and
-        fp32-vector entries (a handful of tiny tensors) are refreshed lazily by `get` / `vec`."""
+        fp32-vector entries (a handful of tiny tensors) are refreshed lazily by `get` / `vec`.  `padded=True`
+        re-casts those padded entries (and the fp32 shadows of the verification arm) now as well, in place, for CUDA
+        graphs that read them without calling `get`."""
         self.epoch += 1
+        if padded:
+            for e in self._c.values():
+                if not e.vec and (not e.plain or e.buf.dtype != torch.bfloat16):
+                    self._cast(e)
         ents = [e for e in self._c.values() if e.plain and not e.vec and e.buf.dtype == torch.bfloat16]
         if not ents or not ents[0].buf.is_cuda:
             return

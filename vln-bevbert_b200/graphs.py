@@ -18,12 +18,15 @@ What makes a step replayable here:
 A graph is keyed by (task, identity and shapes of the batch tensors).  sem / masksem, whose per-item loss has a
 device-computed length, run in the model's `sync_free_mean` mode (mean over a device-side weight, same value and
 gradients); a step whose capture fails (a host synchronisation somewhere in forward) falls back to eager launches.
+
+`GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets.
 """
 import torch
 
 from . import blocks
 from . import kernels as K
 from . import _lib
+from .model import ops
 
 EAGER_TASKS = ()      # every pre-training task is capturable (sem / masksem through the model's sync_free_mean mode)
 
@@ -187,3 +190,205 @@ class GraphedTrainStep:
         """kernels of libbevbert_b200.so inside the captured step of (batch, task), or None when it runs eagerly."""
         ent = self.entries.get(self._sig(batch, task))
         return ent.get("launches") if ent and ent.get("graph") is not None else None
+
+
+# =============================================================================================== agent per-step API
+# Inputs of GlocalTextPathNavCMT.forward(mode, batch) and the dimensions of each that are padded to a multiple of 8 in
+# a graph's static buffers.  Every padding value is zero / False: masks False, ids / features / pair distances 0,
+# visited False, candidate index 0 (cell 0).  The model turns False masks into -10000 (text, map, BEV keys) or -inf
+# (panorama keys) and -inf logits, so real rows see exact zeros from padded slots.
+NAV_PAD_DIMS = {
+    "language": {"txt_ids": (1,), "txt_masks": (1,)},
+    "panorama": {"view_img_fts": (1,), "obj_img_fts": (1,), "loc_fts": (1,), "nav_types": (1,), "view_lens": (),
+                 "obj_lens": ()},
+    "navigation": {"txt_embeds": (1,), "txt_masks": (1,), "gmap_img_embeds": (1,), "gmap_step_ids": (1,),
+                   "gmap_pos_fts": (1,), "gmap_masks": (1,), "gmap_pair_dists": (1, 2), "gmap_visited_masks": (1,),
+                   "bev_fts": (), "bev_pos_fts": (), "bev_masks": (), "bev_nav_masks": (), "bev_cand_idxs": (1,),
+                   "obj_embeds": (1,), "obj_masks": (1,)},
+}
+
+
+def _round8(n):
+    return (n + 7) // 8 * 8
+
+
+def nav_bucket(mode, batch):
+    """Graph key of a per-step call: mode, deterministic flag, and the padded shape and dtype of every input (B, object
+    presence, instruction length, map nodes, BEV candidates, object and panorama tokens)."""
+    key = [mode, torch.are_deterministic_algorithms_enabled()]
+    for name, dims in NAV_PAD_DIMS[mode].items():
+        x = batch.get(name)
+        if x is None:
+            key.append(None)
+        else:
+            key.append((tuple(_round8(n) if d in dims else n for d, n in enumerate(x.shape)), x.dtype))
+    return tuple(key)
+
+
+def nav_pad(mode, batch, device):
+    """The padded inputs a replay of `batch` computes on, as new zero-padded device tensors."""
+    out = {}
+    for name, k in zip(NAV_PAD_DIMS[mode], nav_bucket(mode, batch)[2:]):
+        if k is not None:
+            out[name] = torch.zeros(k[0], dtype=k[1], device=device)
+            out[name][tuple(slice(0, n) for n in batch[name].shape)] = batch[name]
+    return out
+
+
+def nav_slice(mode, out, batch):
+    """Outputs of a padded call cut back to the caller's shapes, as fresh tensors."""
+    c = torch.Tensor.clone
+    if mode == "language":
+        return c(out[:, :batch["txt_ids"].shape[1]])
+    if mode == "panorama":
+        T = batch["loc_fts"].shape[1]            # = the view width, or max(view + object lens) with objects
+        return c(out[0][:, :T]), c(out[1][:, :T])
+    G, Kc = batch["gmap_masks"].shape[1], batch["bev_cand_idxs"].shape[1]
+    res = {"gmap_embeds": c(out["gmap_embeds"][:, :G]), "global_logits": c(out["global_logits"][:, :G]),
+           "local_logits": c(out["local_logits"][:, :Kc]), "fused_logits": c(out["fused_logits"][:, :G]),
+           "obj_logits": None}
+    if out["obj_logits"] is not None:
+        res["obj_logits"] = c(out["obj_logits"][:, :batch["obj_masks"].shape[1]])
+    return res
+
+
+def nav_forward_padded(model, mode, pad, host=None):
+    """model on padded inputs `pad` (nav_pad).  Navigation takes the viewpoint-id lists of the caller's batch in `host`:
+    a (gmap_vpids, bev_cand_vpids) pair, where gmap_vpids may be a PreparedList with staged fusion matches."""
+    if mode == "language":
+        return model.forward_text(pad["txt_ids"], pad["txt_masks"])
+    if mode == "panorama":
+        return model.forward_panorama_per_step(pad["view_img_fts"], pad.get("obj_img_fts"), pad["loc_fts"],
+                                               pad["nav_types"], pad["view_lens"], pad.get("obj_lens"),
+                                               vtot=pad["loc_fts"].shape[1])
+    p = pad
+    return model.forward_navigation_per_step(
+        p["txt_embeds"], p["txt_masks"], p["gmap_img_embeds"], p["gmap_step_ids"], p["gmap_pos_fts"], p["gmap_masks"],
+        p["gmap_pair_dists"], p["gmap_visited_masks"], host[0], p["bev_fts"], p["bev_pos_fts"], p["bev_masks"],
+        p["bev_nav_masks"], p["bev_cand_idxs"], host[1], p.get("obj_embeds"), p.get("obj_masks"))
+
+
+class GraphedNavigation:
+    """The agents' per-step calls `model(mode, batch)` (GlocalTextPathNavCMT: language / panorama / navigation) replayed
+    as CUDA graphs.  Called like the model, with the same inputs and outputs.
+
+    In eval mode under torch.no_grad() each call copies its inputs into the static buffers of its shape bucket
+    (`nav_bucket`: every variable length rounded up to a multiple of 8, zero padding) and replays the bucket's graph,
+    captured at its first call; outputs are sliced back to the caller's shapes as fresh tensors (the agents keep views
+    of them across steps, which a view of a static buffer would not survive).  The SAP fusion matches are host string
+    work: they are written into the bucket's pinned staging buffer before the replay, and the graph's copy node reads
+    them from there.  Training or grad-enabled calls (DAgger rollouts), and buckets whose capture failed, run the model
+    eagerly and unchanged.
+
+    Weights: a replay reads the bf16 weight shadows without `WeightCache.get`, so they are all re-cast in place (one
+    launch, `refresh_all`) at every `language` call -- once per episode -- and before the first replay.  That picks up
+    `load_state_dict` and optimizer steps between validations.  A parameter whose storage moved since a graph was
+    captured (`.to()`, the packed-bias re-homing of `WeightCache.vec`) drops that graph; it is captured again at its
+    next call.  All graphs share one memory pool.  With G <= 100 map nodes there are at most 13 G-buckets per (B,
+    K-bucket).
+
+    Agent side: `vln_bert.vln_bert.forward = GraphedNavigation(vln_bert.vln_bert)` keeps the module, its state_dict and
+    its train / eval switch, and routes its calls here."""
+
+    def __init__(self, model):
+        self.model = model
+        self.params = list(model.parameters())
+        self.entries = {}
+        self.pool = None
+        self.fresh = False
+
+    def _eager(self, mode, batch):
+        return type(self.model).forward(self.model, mode, batch)
+
+    def _param_ptrs(self):
+        return tuple(p.data_ptr() for p in self.params)
+
+    def refresh(self):
+        """Re-cast every weight shadow from the current parameters and drop graphs whose parameters moved."""
+        self.model.rt.wc.refresh_all(padded=True)
+        ptrs = self._param_ptrs()
+        for k in [k for k, e in self.entries.items() if e.get("ptrs") not in (None, ptrs)]:
+            ent = self.entries.pop(k)
+            if ent["stage"] is not None:
+                ent["done"].synchronize()   # its last replay may still have to copy the pinned staging buffer
+        self.fresh = True
+
+    def __call__(self, mode, batch):
+        if self.model.training or torch.is_grad_enabled() or mode not in NAV_PAD_DIMS:
+            return self._eager(mode, batch)
+        if mode == "language" or not self.fresh:
+            self.refresh()
+        key = nav_bucket(mode, batch)
+        ent = self.entries.get(key)
+        if ent is None:
+            ent = self.entries[key] = self._new_entry(mode, batch)
+        if ent["failed"]:
+            return self._eager(mode, batch)
+        self._fill(ent, mode, batch)
+        if ent["graph"] is None:
+            try:
+                self._capture(ent, mode)
+            except Exception as e:          # e.g. a host synchronisation inside forward: this bucket stays eager
+                import warnings
+                warnings.warn("CUDA-graph capture of the %s call failed (%s: %s); running it eagerly" % (
+                    mode, type(e).__name__, str(e)[:200]))
+                torch.cuda.synchronize()
+                ent["failed"] = True
+                return self._eager(mode, batch)
+        ent["graph"].replay()
+        if ent["stage"] is not None:
+            ent["done"].record()
+        return nav_slice(mode, ent["out"], batch)
+
+    def _new_entry(self, mode, batch):
+        dev = self.params[0].device
+        bufs = {}
+        for name, k in zip(NAV_PAD_DIMS[mode], nav_bucket(mode, batch)[2:]):
+            if k is not None:
+                bufs[name] = torch.zeros(k[0], dtype=k[1], device=dev)
+        ent = {"in": bufs, "ext": {}, "graph": None, "out": None, "failed": False, "ptrs": None, "launches": None,
+               "stage": None, "host": None}
+        if mode == "navigation":
+            B, G = bufs["gmap_masks"].shape
+            Kc = bufs["bev_cand_idxs"].shape[1]
+            ent["stage"] = torch.zeros(2, B, G, Kc, dtype=torch.float32, pin_memory=True)
+            ent["done"] = torch.cuda.Event()
+        return ent
+
+    def _fill(self, ent, mode, batch):
+        for name, buf in ent["in"].items():
+            x = batch[name]
+            ext, last = tuple(x.shape), ent["ext"].get(name)
+            if last is not None and any(a < b for a, b in zip(ext, last)):
+                buf.zero_()                 # the previous call of this bucket left real values beyond the new extent
+            buf[tuple(slice(0, n) for n in ext)].copy_(x)
+            ent["ext"][name] = ext
+        if ent["stage"] is not None:
+            # the previous replay of this bucket must have copied the staging buffer before the host rewrites it
+            if ent["graph"] is not None:
+                ent["done"].synchronize()
+            _, B, G, Kc = ent["stage"].shape
+            gv = ops.PreparedList(batch["gmap_vpids"])
+            cands = batch["bev_cand_vpids"]
+            ops._fusion_matches(gv, [c[1:] for c in cands], G, Kc, out=ent["stage"])
+            gv.host_fusion = ((G, Kc), ent["stage"])
+            ent["host"] = (gv, cands)
+
+    def _capture(self, ent, mode):
+        torch.cuda.synchronize()
+        # eager warm-up on the static buffers: weight shadows, packed biases, library workspaces, cuBLAS state
+        nav_forward_padded(self.model, mode, ent["in"], ent["host"])
+        torch.cuda.synchronize()
+        if self.pool is None:
+            self.pool = torch.cuda.graph_pool_handle()
+        g = torch.cuda.CUDAGraph()
+        n0 = K.launch_count()
+        with torch.cuda.graph(g, pool=self.pool):
+            out = nav_forward_padded(self.model, mode, ent["in"], ent["host"])
+        ent["launches"] = K.launch_count() - n0
+        ent["graph"], ent["out"], ent["ptrs"] = g, out, self._param_ptrs()
+
+    def launches(self, mode, batch):
+        """kernels of libbevbert_b200.so inside the graph of this call's bucket, or None when it runs eagerly."""
+        ent = self.entries.get(nav_bucket(mode, batch))
+        return ent["launches"] if ent is not None and ent["graph"] is not None else None

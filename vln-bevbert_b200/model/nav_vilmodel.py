@@ -43,12 +43,13 @@ class GlocalTextPathNavCMT(PreTrainedBase):
         rt.begin(self.training)
         return Bk.to_f32(self.lang_encoder(rt, self.embeddings(rt, txt_ids), txt_masks))
 
-    def forward_panorama_per_step(self, view_img_fts, obj_img_fts, loc_fts, nav_types, view_lens, obj_lens):
+    def forward_panorama_per_step(self, view_img_fts, obj_img_fts, loc_fts, nav_types, view_lens, obj_lens, vtot=None):
+        """`vtot`: token width with objects (see ImageEmbeddings.forward); None reads max(view + object lens)."""
         rt = self.rt
         rt.begin(self.training)
         rt.feat_p = 0.0          # the agents apply feature dropout themselves (map_nav_src/models/model.py:21-41)
         emb, lens = self.img_embeddings(rt, view_img_fts, obj_img_fts, loc_fts, nav_types, None, view_lens, obj_lens,
-                                        self.embeddings.token_type_embeddings)
+                                        self.embeddings.token_type_embeddings, vtot=vtot)
         return Bk.to_f32(emb), gen_seq_masks(lens, emb.shape[1])
 
     def forward_navigation_per_step(self, txt_embeds, txt_masks, gmap_img_embeds, gmap_step_ids, gmap_pos_fts,

@@ -147,20 +147,22 @@ def prepare_batch(batch, wire_dtype=None):
     return out
 
 
-def _fusion_matches(gmap_vpids, last_cand_vpids, G, Kc):
-    """(2,B,G,Kc) host matrix: [0] every (node j == candidate k) match, [1] only the last candidate per viewpoint."""
+def _fusion_matches(gmap_vpids, last_cand_vpids, G, Kc, out=None):
+    """(2,B,G,Kc) host matrix: [0] every (node j == candidate k) match, [1] only the last candidate per viewpoint.
+    `out`: an fp32 host tensor of that shape to fill instead of a new one (a pinned staging buffer)."""
     B = len(gmap_vpids)
-    E2 = torch.zeros(2, B, G, Kc, dtype=torch.float32)
+    E2 = torch.zeros(2, B, G, Kc, dtype=torch.float32) if out is None else out.zero_()
+    e = E2.numpy()                                        # element writes through numpy: no torch op per match
     for i in range(B):
         pos = {vp: j for j, vp in enumerate(gmap_vpids[i]) if j > 0}
         last = {}
         for k, vp in enumerate(last_cand_vpids[i]):
             j = pos.get(vp)
             if j is not None and k + 1 < Kc:
-                E2[0, i, j, k + 1] = 1.0
+                e[0, i, j, k + 1] = 1.0
                 last[vp] = (j, k + 1)                     # `tmp[cand_vpid] = ...` overwrites: the last view wins
         for j, k in last.values():
-            E2[1, i, j, k] = 1.0
+            e[1, i, j, k] = 1.0
     return E2
 
 
@@ -174,6 +176,10 @@ def build_sap_fusion(gmap_vpids, gmap_visited_masks, last_cand_vpids, G, Kc, dev
     pre = getattr(gmap_vpids, "host_fusion", None)
     E2 = pre[1] if (pre is not None and pre[0] == (G, Kc)) else _fusion_matches(gmap_vpids, last_cand_vpids, G, Kc)
     if device.type == "cuda" and not E2.is_pinned():
+        if torch.cuda.is_current_stream_capturing():
+            # a graph would re-read this temporary host buffer at every replay, long after it was freed
+            raise RuntimeError("build_sap_fusion under CUDA-graph capture needs the fusion matches staged in a pinned "
+                               "buffer (PreparedList.host_fusion)")
         E2 = E2.pin_memory()
     E2 = E2.to(device, non_blocking=True)
     vis = gmap_visited_masks.to(torch.float32)                     # (B,G)

@@ -269,9 +269,11 @@ class ImageEmbeddings(nn.Module):  # vilmodel.py:465-536
         self.pano_encoder = TransformerEncoder(config, config.num_pano_layers) if config.num_pano_layers > 0 else None
 
     def forward(self, rt, traj_view_img_fts, traj_obj_img_fts, traj_loc_fts, traj_nav_types, traj_step_lens,
-                traj_vp_view_lens, traj_vp_obj_lens, type_embed_layer):
+                traj_vp_view_lens, traj_vp_obj_lens, type_embed_layer, vtot=None):
         """-> (traj_embeds (sumP, Vtot, H) flat over panoramas, traj_vp_lens (sumP,)); the reference returns
-        the same data split per sample (torch.split by traj_step_lens)."""
+        the same data split per sample (torch.split by traj_step_lens).  With objects, Vtot is max(view + object
+        lens), read from the device; a caller that knows a width >= that (the padded width of `traj_loc_fts`) passes it
+        as `vtot`, which keeps the call free of host synchronisations (CUDA-graph capture)."""
         dev = traj_view_img_fts.device
         lin_ln = lambda x, lin, ln, p_in=0.0: Bk.run_block(Bk.LinearLNImpl(rt, 1e-12, p_in), [x], _wb(lin) + _wb(ln))
         view = lin_ln(traj_view_img_fts, self.img_linear, self.img_layer_norm, rt.feat_p)
@@ -283,7 +285,7 @@ class ImageEmbeddings(nn.Module):  # vilmodel.py:465-536
             nP, V, Hd = view.shape
             O = obj.shape[1]
             lens = traj_vp_view_lens + traj_vp_obj_lens
-            Vtot = int(lens.max())
+            Vtot = int(lens.max()) if vtot is None else vtot
             ar = torch.arange(Vtot, device=dev)[None, :]
             base = torch.arange(nP, device=dev)[:, None]
             vl, ol = traj_vp_view_lens[:, None], traj_vp_obj_lens[:, None]
