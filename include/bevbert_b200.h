@@ -146,6 +146,29 @@ int bb_bev_scatter_sem_f64(const double* sems, const int32_t* cell_idx, int B, i
 int bb_bev_scatter_sem_u8(const uint8_t* sem_ids, const int32_t* cell_idx, int B, int P, int S, int ncell, double* bev_sem,
                           uint8_t* sem_mask, void* stream);
 
+/* Agent-side BEV straight from the per-node point clouds of the navigation graph (map_nav_src/r2r/agent.py:293-337:
+ * GraphMap.gather_node_pc -> pad_sequence -> splat -> project_bev, without the concatenation and padding copies).
+ * One row per node (32 bytes): world-frame points f32 (n, 3), no-depth mask u8/bool (n) or NULL, features (n, C) f32 or
+ * bf16 (feat_bf16 = 1; rows 16- resp. 8-byte aligned), n >= 0.  Sample b takes the nodes sample_nodes[b] ..
+ * sample_nodes[b+1]-1 (B+1 non-decreasing offsets) in that order, the order the reference concatenates them; a node
+ * may appear in several samples.  Per point: p = pc - S_w2c[b], e_j = ((p0 E_j0 + p1 E_j1) + p2 E_j2) + E_j3 with
+ * E = T_w2c[b] (4x4 row major), one rounding per operation; the cell index of bb_bev_cell_index; then the
+ * scatter-mean of bb_bev_scatter_mean_f32 over the concatenated cloud (points of a cell added in ascending
+ * concatenated order, no atomics, no limit on the points per sample).  bev f32 (B, D*D, C), ob_mask u8 (B, D*D);
+ * a sample without nodes gives zeros and a false mask.
+ * nodes and sample_nodes are HOST arrays: they are validated, then copied on `stream` into table_dev (device,
+ * 8-byte aligned, n_nodes*32 + (B+1)*4 bytes: the rows, then the offsets), which the kernel reads.  From pinned memory
+ * the copy is asynchronous and the host arrays must stay unchanged until the stream has executed it. */
+typedef struct bb_bev_node {
+  const float* pc;
+  const uint8_t* no_depth;
+  const void* feat;
+  int64_t n;
+} bb_bev_node;
+int bb_bev_splat_nodes(const bb_bev_node* nodes, int n_nodes, const int32_t* sample_nodes, int B, void* table_dev,
+                       const float* S_w2c, const float* T_w2c, int C, int feat_bf16, int map_dim, float map_res,
+                       float y_clip, float* bev, uint8_t* ob_mask, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Row kernels (coalesced, vectorised, warp reductions; fp32 math, bf16 storage).
  * ------------------------------------------------------------------------------------------- */

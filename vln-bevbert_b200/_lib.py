@@ -113,6 +113,8 @@ _SIGNATURES = {
     "bb_bev_scatter_mean_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int] + [c_void_p] * 5),
     "bb_bev_scatter_sem_f64": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "bb_bev_scatter_sem_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "bb_bev_splat_nodes": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                   c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "bb_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_u64, c_u32, c_float, c_void_p]),
     "bb_cast_bf16_f32": (c_int, [c_void_p, c_void_p, c_i64, c_void_p]),
     "bb_layernorm_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_i64, c_int,

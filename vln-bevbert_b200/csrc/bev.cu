@@ -16,10 +16,37 @@
 namespace bb {
 
 // ---------------------------------------------------------------------------------------------
-// One thread per point. All arithmetic uses explicit round-to-nearest single operations (no FMA
-// contraction) in a fixed order so that the CPU oracle (oracle/bevbert_ref.py: lift_points, cell_index) reproduces
-// every bit.
+// Point arithmetic shared by every kernel that places points into the map. All of it uses explicit round-to-nearest
+// single operations (no FMA contraction) in a fixed order so that the CPU oracles (oracle/bevbert_ref.py: lift_points,
+// cell_index; tests/nav_bev_oracle.py: nav_splat_nodes) reproduce every bit.
 // ---------------------------------------------------------------------------------------------
+// world -> ego: (w - S) then [p, 1] * T_w2c^T, each 4-term dot product left to right (pretrain_cmt.py:133-137,
+// map_nav_src/r2r/agent.py:162-166). S (3), E = T_w2c (4x4 row major).
+__device__ __forceinline__ void ego_transform(float w0, float w1, float w2, const float* S, const float* E, float e[3]) {
+  const float p0 = __fsub_rn(w0, S[0]), p1 = __fsub_rn(w1, S[1]), p2 = __fsub_rn(w2, S[2]);
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    float acc = __fmul_rn(p0, E[j * 4 + 0]);
+    acc = __fadd_rn(acc, __fmul_rn(p1, E[j * 4 + 1]));
+    acc = __fadd_rn(acc, __fmul_rn(p2, E[j * 4 + 2]));
+    acc = __fadd_rn(acc, E[j * 4 + 3]);
+    e[j] = acc;
+  }
+}
+
+// discretise an ego-frame point (bev_utils.py:393-406): round half to even, bounds, height clip -> D*z+x or -1.
+// NaN coordinates compare false everywhere in the reference and then index out of range; we drop them.
+__device__ __forceinline__ int32_t bev_cell(float e0, float e1, float e2, bool no_depth, int D, float res, float half,
+                                            float y_clip) {
+  const float gx = rintf(__fadd_rn(__fdiv_rn(e0, res), half));
+  const float gz = rintf(__fadd_rn(__fdiv_rn(e2, res), half));
+  const float Df = (float)D;
+  const bool outside = (gx >= Df) || (gz >= Df) || (gx < 0.0f) || (gz < 0.0f);
+  const bool bad = no_depth || outside || (e1 > y_clip) || !(gx == gx) || !(gz == gz);
+  return bad ? -1 : (int32_t)(Df * gz + gx);
+}
+
+// One thread per point.
 __global__ void lift_index_kernel(const float* __restrict__ depths, const float* __restrict__ T_c2w,
                                   const float* __restrict__ S_w2c, const float* __restrict__ T_w2c, int B, int V, int Hf,
                                   int Wf, float depth_scale, float fx, float fy, float cx, float cy, int D, float res,
@@ -52,33 +79,14 @@ __global__ void lift_index_kernel(const float* __restrict__ depths, const float*
     acc = __fadd_rn(acc, T[j * 4 + 3]);
     w[j] = acc;
   }
-  // world -> ego: (pc - S) then [pc,1] * T_w2c^T   (pretrain_cmt.py:133-137)
-  const float* S = S_w2c + (long long)b * 3;
-  const float p0 = __fsub_rn(w[0], S[0]), p1 = __fsub_rn(w[1], S[1]), p2 = __fsub_rn(w[2], S[2]);
-  const float* E = T_w2c + (long long)b * 16;
   float e[3];
-#pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    float acc = __fmul_rn(p0, E[j * 4 + 0]);
-    acc = __fadd_rn(acc, __fmul_rn(p1, E[j * 4 + 1]));
-    acc = __fadd_rn(acc, __fmul_rn(p2, E[j * 4 + 2]));
-    acc = __fadd_rn(acc, E[j * 4 + 3]);
-    e[j] = acc;
-  }
+  ego_transform(w[0], w[1], w[2], S_w2c + (long long)b * 3, T_w2c + (long long)b * 16, e);
   if (pc_out) {
     pc_out[gid * 3 + 0] = e[0];
     pc_out[gid * 3 + 1] = e[1];
     pc_out[gid * 3 + 2] = e[2];
   }
-  // discretise (bev_utils.py:393-406): round half to even, bounds, height clip
-  const float gx = rintf(__fadd_rn(__fdiv_rn(e[0], res), half));
-  const float gz = rintf(__fadd_rn(__fdiv_rn(e[2], res), half));
-  const float Df = (float)D;
-  const bool outside = (gx >= Df) || (gz >= Df) || (gx < 0.0f) || (gz < 0.0f);
-  const bool above = e[1] > y_clip;
-  // NaN coordinates compare false everywhere in the reference and then index out of range; we drop them.
-  const bool bad = no_depth || outside || above || !(gx == gx) || !(gz == gz);
-  cell_idx[gid] = bad ? -1 : (int32_t)(Df * gz + gx);
+  cell_idx[gid] = bev_cell(e[0], e[1], e[2], no_depth, D, res, half, y_clip);
 }
 
 // Cell index of an ego-frame point cloud (PointCloud.project_bev called with a ready-made cloud: the agents gather
@@ -89,13 +97,8 @@ __global__ void cell_index_kernel(const float* __restrict__ pc, const uint8_t* _
   bb::pdl_trigger();
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (gid >= n) return;
-  const float e0 = pc[gid * 3 + 0], e1 = pc[gid * 3 + 1], e2 = pc[gid * 3 + 2];
-  const float gx = rintf(__fadd_rn(__fdiv_rn(e0, res), half));
-  const float gz = rintf(__fadd_rn(__fdiv_rn(e2, res), half));
-  const float Df = (float)D;
-  const bool outside = (gx >= Df) || (gz >= Df) || (gx < 0.0f) || (gz < 0.0f);
-  const bool bad = (no_depth && no_depth[gid]) || outside || (e1 > y_clip) || !(gx == gx) || !(gz == gz);
-  cell_idx[gid] = bad ? -1 : (int32_t)(Df * gz + gx);
+  cell_idx[gid] = bev_cell(pc[gid * 3 + 0], pc[gid * 3 + 1], pc[gid * 3 + 2], no_depth && no_depth[gid], D, res, half,
+                           y_clip);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -240,6 +243,125 @@ scatter_sem_f64_kernel(const double* __restrict__ sems, const int32_t* __restric
   if (lane == 0 && sem_mask) sem_mask[(long long)b * ncell + cell] = tot > 0.0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Agent-side BEV straight from the node point clouds (map_nav_src/r2r/agent.py:293-337: gather_node_pc -> pad_sequence
+// -> splat -> project_bev). Block = 8 warps = 8 cells of one sample, as in scatter_mean_f32_kernel. The block walks
+// the sample's nodes in table order and, inside them, the points in row order, SN_CHUNK at a time: all threads
+// ego-transform and discretise a chunk into shared memory (cell index + feature row pointer per point), then each warp
+// ballot-scans the chunk for its cell and adds the matching rows. The sums and counts stay in registers across chunks
+// and nodes, so the points of a cell are added in ascending order of the concatenated cloud, with no limit on the
+// number of points. Columns beyond SC_MAXV * 128 take further passes over the whole walk.
+// ---------------------------------------------------------------------------------------------
+constexpr int SN_CHUNK = 2048;
+
+template <typename FT>
+__global__ void __launch_bounds__(SC_WARPS * 32)
+splat_nodes_kernel(const bb_bev_node* __restrict__ nodes, const int32_t* __restrict__ sample_nodes,
+                   const float* __restrict__ S_w2c, const float* __restrict__ T_w2c, int C, int D, float res, float half,
+                   float y_clip, float* __restrict__ bev, uint8_t* __restrict__ ob_mask) {
+  __shared__ int32_t scell[SN_CHUNK];
+  __shared__ const FT* srow[SN_CHUNK];
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  const int b = blockIdx.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ncell = D * D;
+  const int cell = blockIdx.x * SC_WARPS + warp;  // a warp past the last cell still stages points
+  const int k0 = sample_nodes[b], k1 = sample_nodes[b + 1];
+  float S[3], E[12];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) S[i] = __ldg(S_w2c + b * 3 + i);
+#pragma unroll
+  for (int i = 0; i < 12; ++i) E[i] = __ldg(T_w2c + b * 16 + i);
+  const long long orow = ((long long)b * ncell + cell) * C;
+
+  float vmax = -INFINITY, vmin = INFINITY;
+  for (int c0 = 0; c0 < C; c0 += SC_MAXV * 128) {
+    float4 acc[SC_MAXV];
+#pragma unroll
+    for (int i = 0; i < SC_MAXV; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    int cnt = 0;
+    int k = k0;
+    long long r = 0;  // next row of node k
+    while (k < k1) {
+      int filled = 0;
+      while (k < k1 && filled < SN_CHUNK) {  // block-uniform: every thread walks the same cursor
+        const long long n = nodes[k].n;
+        const int take = (int)min(n - r, (long long)(SN_CHUNK - filled));
+        if (take > 0) {
+          const float* pc = nodes[k].pc;
+          const uint8_t* nod = nodes[k].no_depth;
+          const FT* ft = reinterpret_cast<const FT*>(nodes[k].feat);
+          for (int i = threadIdx.x; i < take; i += blockDim.x) {
+            const long long row = r + i;
+            float e[3];
+            ego_transform(pc[row * 3 + 0], pc[row * 3 + 1], pc[row * 3 + 2], S, E, e);
+            scell[filled + i] = bev_cell(e[0], e[1], e[2], nod && nod[row], D, res, half, y_clip);
+            srow[filled + i] = ft + row * C;
+          }
+          filled += take;
+          r += take;
+        }
+        if (r >= n) {
+          ++k;
+          r = 0;
+        }
+      }
+      __syncthreads();
+      if (cell < ncell) {
+        for (int base = 0; base < filled; base += 32) {
+          const int my = (base + lane < filled) ? scell[base + lane] : -1;
+          unsigned m = __ballot_sync(0xffffffffu, my == cell);
+          while (m) {
+            const int j = __ffs(m) - 1;
+            m &= m - 1;
+            const FT* rowp = srow[base + j] + c0;
+            float4 t[SC_MAXV];
+#pragma unroll
+            for (int i = 0; i < SC_MAXV; ++i) {
+              const int col = i * 128 + lane * 4;
+              t[i] = (c0 + col < C) ? load_feat4(rowp + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int i = 0; i < SC_MAXV; ++i) {
+              acc[i].x = __fadd_rn(acc[i].x, t[i].x);
+              acc[i].y = __fadd_rn(acc[i].y, t[i].y);
+              acc[i].z = __fadd_rn(acc[i].z, t[i].z);
+              acc[i].w = __fadd_rn(acc[i].w, t[i].w);
+            }
+            ++cnt;
+          }
+        }
+      }
+      __syncthreads();  // the next chunk overwrites the staging arrays
+    }
+    if (cell < ncell) {
+      const float denom = (float)(cnt < 1 ? 1 : cnt);  // count.clamp(min=1)
+#pragma unroll
+      for (int i = 0; i < SC_MAXV; ++i) {
+        const int col = c0 + i * 128 + lane * 4;
+        if (col < C) {
+          float4 mval;
+          mval.x = __fdiv_rn(acc[i].x, denom);
+          mval.y = __fdiv_rn(acc[i].y, denom);
+          mval.z = __fdiv_rn(acc[i].z, denom);
+          mval.w = __fdiv_rn(acc[i].w, denom);
+          vmax = fmaxf(vmax, fmaxf(fmaxf(mval.x, mval.y), fmaxf(mval.z, mval.w)));
+          vmin = fminf(vmin, fminf(fminf(mval.x, mval.y), fminf(mval.z, mval.w)));
+          *reinterpret_cast<float4*>(bev + orow + col) = mval;
+        }
+      }
+    }
+  }
+  if (cell >= ncell) return;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
+    vmin = fminf(vmin, __shfl_xor_sync(0xffffffffu, vmin, o));
+  }
+  if (lane == 0) ob_mask[(long long)b * ncell + cell] = !((vmax == 0.0f) && (vmin == 0.0f));
+}
+
 }  // namespace bb
 
 extern "C" int bb_bev_lift_index(const float* depths, const float* T_c2w, const float* S_w2c, const float* T_w2c, int B,
@@ -362,4 +484,51 @@ extern "C" int bb_bev_scatter_sem_f64(const double* sems, const int32_t* cell_id
                                                                                     bev_sem, sem_mask);
   count_launch();
   return check_launch("scatter_sem_f64_kernel");
+}
+
+extern "C" int bb_bev_splat_nodes(const bb_bev_node* nodes, int n_nodes, const int32_t* sample_nodes, int B,
+                                  void* table_dev, const float* S_w2c, const float* T_w2c, int C, int feat_bf16,
+                                  int map_dim, float map_res, float y_clip, float* bev, uint8_t* ob_mask, void* stream) {
+  using namespace bb;
+  if (B < 0 || n_nodes < 0) return set_error("bb_bev_splat_nodes: B and n_nodes must be >= 0");
+  if (B > 65535) return set_error("bb_bev_splat_nodes: at most 65535 samples per call");
+  if (!sample_nodes || !table_dev || !S_w2c || !T_w2c || !bev || !ob_mask || (n_nodes > 0 && !nodes))
+    return set_error("bb_bev_splat_nodes: null argument");
+  if (C <= 0 || C % 4 != 0) return set_error("bb_bev_splat_nodes: C must be a positive multiple of 4");
+  if (map_dim <= 0 || map_dim > 46340) return set_error("bb_bev_splat_nodes: map_dim out of range");
+  if ((uintptr_t)table_dev % 8 != 0) return set_error("bb_bev_splat_nodes: table_dev must be 8-byte aligned");
+  if (sample_nodes[0] < 0 || sample_nodes[B] > n_nodes)
+    return set_error("bb_bev_splat_nodes: sample_nodes must lie in [0, n_nodes]");
+  for (int b = 0; b < B; ++b)
+    if (sample_nodes[b + 1] < sample_nodes[b]) return set_error("bb_bev_splat_nodes: sample_nodes must be non-decreasing");
+  const uintptr_t feat_align = feat_bf16 ? 8 : 16;  // 4 features per load: one 8- or 16-byte access
+  for (int i = 0; i < n_nodes; ++i) {
+    const bb_bev_node& nd = nodes[i];
+    if (nd.n < 0) return set_error("bb_bev_splat_nodes: negative node size");
+    if (nd.n == 0) continue;
+    if (!nd.pc || !nd.feat) return set_error("bb_bev_splat_nodes: null point or feature pointer in a node");
+    if ((uintptr_t)nd.pc % 4 != 0) return set_error("bb_bev_splat_nodes: misaligned point rows");
+    if ((uintptr_t)nd.feat % feat_align != 0) return set_error("bb_bev_splat_nodes: misaligned feature rows");
+  }
+  if (B == 0) return 0;
+  const cudaStream_t st = (cudaStream_t)stream;
+  char* tab = static_cast<char*>(table_dev);
+  const size_t rows_bytes = (size_t)n_nodes * sizeof(bb_bev_node);
+  if (rows_bytes && cudaMemcpyAsync(tab, nodes, rows_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return check_launch("bb_bev_splat_nodes: table copy");
+  if (cudaMemcpyAsync(tab + rows_bytes, sample_nodes, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return check_launch("bb_bev_splat_nodes: offsets copy");
+  const int ncell = map_dim * map_dim;
+  const float half = (float)((map_dim - 1) / 2.0);
+  dim3 grid((ncell + SC_WARPS - 1) / SC_WARPS, B);
+  const bb_bev_node* dnodes = reinterpret_cast<const bb_bev_node*>(tab);
+  const int32_t* doffs = reinterpret_cast<const int32_t*>(tab + rows_bytes);
+  if (feat_bf16)
+    bb::launch_pdl(splat_nodes_kernel<__nv_bfloat16>, grid, SC_WARPS * 32, 0, st, dnodes, doffs, S_w2c, T_w2c, C,
+                   map_dim, map_res, half, y_clip, bev, ob_mask);
+  else
+    bb::launch_pdl(splat_nodes_kernel<float>, grid, SC_WARPS * 32, 0, st, dnodes, doffs, S_w2c, T_w2c, C, map_dim,
+                   map_res, half, y_clip, bev, ob_mask);
+  count_launch();
+  return check_launch("splat_nodes_kernel");
 }

@@ -5,6 +5,7 @@ import math
 
 import torch
 
+from .. import bev_nodes
 from .. import kernels as K
 
 
@@ -65,20 +66,25 @@ class PointCloud:
         and agent-side `project_bev(pc, mask, feat)` -> (bevs, ob_masks) (map_nav_src/models/bev_utils.py:382-417,
         called at map_nav_src/r2r/agent.py:170).  pc (B,N,3) ego-frame points, no_depth_mask (B,N) bool, pc_feat
         (B,N,C) fp32, pc_sem (B,N,S) fp64 one-hots.  Ragged inputs (a python list of per-sample tensors, as the agents
-        build them from neighbouring panoramas) are padded with no-depth points."""
+        build them from neighbouring panoramas) are pooled where they lie, one node per sample with the identity ego
+        transform (`splat_nodes`): the same result as padding them with no-depth points.  With semantics they are
+        padded that way."""
         if isinstance(pc, (list, tuple)):
-            n = max(x.shape[0] for x in pc)
+            if pc_sem is not None:
+                pad = torch.nn.utils.rnn.pad_sequence
+                return self.project_bev(pad(list(pc), batch_first=True),
+                                        pad([m.bool() for m in no_depth_mask], batch_first=True, padding_value=True),
+                                        pad(list(pc_feat), batch_first=True), pad(list(pc_sem), batch_first=True))
+            B = len(pc)
             dev = pc[0].device
-
-            def pad(xs, fill=0):
-                out = xs[0].new_full((len(xs), n) + tuple(xs[0].shape[1:]), fill)
-                for i, x in enumerate(xs):
-                    out[i, :x.shape[0]] = x
-                return out
-            no_depth_mask = pad([m.bool() for m in no_depth_mask], True)
-            pc, pc_feat = pad(list(pc)), pad(list(pc_feat))
-            pc_sem = pad(list(pc_sem)) if pc_sem is not None else None
-            del dev
+            S = torch.zeros(B, 3, dtype=torch.float32, device=dev)
+            T = torch.eye(4, dtype=torch.float32, device=dev).expand(B, 4, 4)
+            clouds = [[(p.float().contiguous(), m.bool().contiguous(),
+                        (f if f.dtype == torch.bfloat16 else f.float()).contiguous())]
+                      for p, m, f in zip(pc, no_depth_mask, pc_feat)]
+            bev, ob = self.splat_nodes(clouds, S, T)
+            D = self.map_dim
+            return bev.view(B, D, D, -1), ob
         D = self.map_dim
         B = pc.shape[0]
         idx = K.bev_cell_index(pc.float(), no_depth_mask, D, self.map_res, self.z_clip_threshold)
@@ -87,6 +93,20 @@ class PointCloud:
         if pc_sem is None:
             return bevs, ob_masks
         return bevs, ob_masks, sem.view(B, D, D, -1), sem_mask.view(B, D, D)
+
+    @torch.no_grad()
+    def splat_nodes(self, clouds, S_w2c, T_w2c):
+        """Agent-side BEV straight from the navigation graph's node clouds: `clouds[b]` is the list of
+        `(pc, pc_mask, pc_feat)` tuples that `GraphMap.node_pc` holds for the nodes sample b gathers, in gather order
+        (world-frame points (n,3), no-depth mask (n,), features (n,C) fp32 or bf16, as `forward` and the agents' `lift`
+        produce them); S_w2c (B,3), T_w2c (B,4,4) the agents' ego transform.  One kernel replaces
+        `GraphMap.gather_node_pc` + `pad_sequence` + `splat` + `project_bev` (map_nav_src/r2r/agent.py:143-192,293-330)
+        with the same result bit for bit, given the fixed-order ego transform.
+        -> (bev_fts (B, D*D, C) fp32, ob_masks (B, D, D) bool)."""
+        D = self.map_dim
+        bev, ob = bev_nodes.bev_splat_nodes(clouds, S_w2c.reshape(-1, 3), T_w2c.reshape(-1, 4, 4), D, self.map_res,
+                                            self.z_clip_threshold)
+        return bev, ob.view(-1, D, D)
 
     @torch.no_grad()
     def splat(self, cell_idx, pc_feat, pc_sem=None, want_bf16=False):
