@@ -171,6 +171,9 @@ int bb_bev_splat_nodes(const bb_bev_node* nodes, int n_nodes, const int32_t* sam
 
 /* ---------------------------------------------------------------------------------------------
  * Row kernels (coalesced, vectorised, warp reductions; fp32 math, bf16 storage).
+ * Every row-matrix and vector pointer of the entry points below that read or write 16-byte vectors (LayerNorm forward /
+ * backward, bb_add_rows, bb_gather_rows_bf16, bb_segment_wsum / _bwd, bb_embed_sum, bb_colsum_bf16 when ld % 8 == 0,
+ * the casts, bb_scatter_rows_sorted) must be 16-byte aligned; a misaligned one is rejected with an error, nothing runs.
  * ------------------------------------------------------------------------------------------- */
 /* f32 -> bf16 cast with optional inverted dropout (nn.Dropout on inputs, pretrain_cmt.py:102-106).
  * drop_thresh = p * 2^32 (0 = no dropout); scale = 1/(1-p). Element index is the RNG counter. */
@@ -181,7 +184,7 @@ int bb_cast_bf16_f32(const void* src, float* dst, int64_t n, void* stream);
 /* y = LayerNorm( dropout(x) + residual ) * gamma + beta, optional output dropout
  * (BertSelfOutput / BertOutput vilmodel.py:150-154,189-193; BertEmbeddings :75-76; nn.LayerNorm sites).
  * x bf16 or f32 (rows, H); residual bf16 or NULL; y bf16; y_f32 optional f32 copy; mean/rstd f32 (rows)
- * saved for backward. H % 8 == 0, H <= 4096. */
+ * saved for backward. H % 8 == 0, H <= 1024. */
 int bb_layernorm_fwd(const void* x, int x_f32, const void* residual, const float* gamma, const float* beta,
                      float eps, int64_t rows, int H, uint64_t seed_in, uint32_t thresh_in, float scale_in,
                      uint64_t seed_out, uint32_t thresh_out, float scale_out, void* y, float* y_f32, float* mean,
@@ -195,7 +198,7 @@ int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x_f32, const
                      float scale_in, uint64_t seed_out, uint32_t thresh_out, float scale_out, void* dx, int dx_f32,
                      void* dres, float* dgamma, float* dbeta, float* dxsum, void* stream);
 
-/* Column sums of a bf16 (rows, N) matrix accumulated into f32 out[N] (bias gradients). */
+/* Column sums of a bf16 (rows, N) matrix with row stride ld accumulated into f32 out[N] (bias gradients). */
 int bb_colsum_bf16(const void* x, int64_t rows, int N, int64_t ld, float* out, void* stream);
 
 /* Masked softmax over the last dim (vilmodel.py:117-127, 335-346; transformer.py MHA):

@@ -8,6 +8,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <initializer_list>
+
 #include "../../include/bevbert_b200.h"
 #include "common.h"
 #include "ptx.cuh"
@@ -880,6 +882,13 @@ static inline unsigned grid1d(long long n, int per_block, int cap = 0) {
   return (unsigned)g;
 }
 
+// every pointer of an entry point whose kernel reads or writes it in 16-byte vectors (NULL counts as aligned)
+static inline bool aligned16(std::initializer_list<const void*> ps) {
+  for (const void* p : ps)
+    if (reinterpret_cast<uintptr_t>(p) & 15) return false;
+  return true;
+}
+
 }  // namespace bb
 
 using namespace bb;
@@ -941,6 +950,7 @@ extern "C" int bb_add_rows(const void* a, const void* b, const float* table, con
   if (rows <= 0) return 0;
   if (H % 8 != 0) return set_error("bb_add_rows: H must be a multiple of 8");
   if (table && !idx) return set_error("bb_add_rows: table needs idx");
+  if (!aligned16({a, b, table, vec, out})) return set_error("bb_add_rows: a / b / table / vec / out must be 16-byte aligned");
   const long long n = rows * (H / 8);
   ACT_T(bb::launch_pdl(add_rows_kernel<T>, (unsigned)((n + 255) / 256), 256, 0, STREAM, (const T*)a, (const T*)b, table, idx, vec,
                                                                    rows, H, (T*)out));
@@ -958,6 +968,7 @@ extern "C" int bb_segment_wsum(const void* src, const int32_t* seg_off, const in
                                int64_t nseg, int H, void* out, void* stream) {
   if (nseg <= 0) return 0;
   if (H % 8 != 0) return set_error("bb_segment_wsum: H must be a multiple of 8");
+  if (!aligned16({src, out})) return set_error("bb_segment_wsum: src / out must be 16-byte aligned");
   ACT_T(bb::launch_pdl(segment_wsum_kernel<T>, (unsigned)((nseg + 7) / 8), 256, 0, STREAM, (const T*)src, seg_off, idx, w, nseg, H,
                                                                       (T*)out));
   count_launch();
@@ -967,6 +978,7 @@ extern "C" int bb_segment_wsum_bwd(const void* dout, const int32_t* seg_off, con
                                    int64_t nseg, int H, float* dsrc_f32, void* stream) {
   if (nseg <= 0) return 0;
   if (H % 8 != 0) return set_error("bb_segment_wsum_bwd: H must be a multiple of 8");
+  if (!aligned16({dout})) return set_error("bb_segment_wsum_bwd: dout must be 16-byte aligned");
   if (det_on()) return set_error("bb_segment_wsum_bwd adds with atomics; in deterministic mode use bb_scatter_rows_sorted");
   ACT_T(bb::launch_pdl(segment_wsum_bwd_kernel<T>, (unsigned)((nseg + 7) / 8), 256, 0, STREAM, (const T*)dout, seg_off, idx, w, nseg, H,
                                                                           dsrc_f32));
@@ -986,6 +998,8 @@ extern "C" int bb_layernorm_fwd(const void* x, int x_f32, const void* residual, 
                                 float* mean, float* rstd, void* stream) {
   if (rows <= 0) return 0;
   if (H % 8 != 0 || H > LN_MAXCH * 256) return set_error("bb_layernorm_fwd: H must be a multiple of 8 and <= 1024");
+  if (!aligned16({x, residual, gamma, beta, y, y_f32}))
+    return set_error("bb_layernorm_fwd: x / residual / gamma / beta / y / y_f32 must be 16-byte aligned");
   const unsigned grid = (unsigned)((rows + LN_WARPS - 1) / LN_WARPS);
   if (x_f32)
     ACT_T(bb::launch_pdl(layernorm_fwd_kernel<float, T>, grid, LN_WARPS * 32, 0, STREAM, 
@@ -1006,6 +1020,8 @@ extern "C" int bb_layernorm_bwd(const void* dy, int dy_f32, const void* x, int x
                                 float* dbeta, float* dxsum, void* stream) {
   if (rows <= 0) return 0;
   if (H % 8 != 0 || H > LN_MAXCH * 256) return set_error("bb_layernorm_bwd: H must be a multiple of 8 and <= 1024");
+  if (!aligned16({dy, x, residual, gamma, dx, dres}))
+    return set_error("bb_layernorm_bwd: dy / x / residual / gamma / dx / dres must be 16-byte aligned");
   long long g = (rows + LN_WARPS - 1) / LN_WARPS;
   if (g > device_sms()) g = device_sms();   // one resident block per SM (233 registers), rows grid-strided
   const unsigned grid = (unsigned)g;
@@ -1052,6 +1068,8 @@ namespace bb {
 template <typename T>
 static int colsum_run(const T* x, long long rows, int N, long long ld, float* out, cudaStream_t stream) {
   if (rows <= 0 || N <= 0) return 0;
+  if (ld % 8 == 0 && !aligned16({x}))      // the kernel reads 16-byte vectors exactly when ld % 8 == 0
+    return set_error("bb_colsum_bf16: x must be 16-byte aligned when ld is a multiple of 8");
   long long gy = (rows + 63) / 64;
   if (gy > 64) gy = 64;
   dim3 grid((N + 255) / 256, (unsigned)gy);
@@ -1133,6 +1151,7 @@ extern "C" int bb_embed_sum(const int64_t* ids, const float* word, const float* 
                             int L, int H, float* out, void* stream) {
   if (ntok <= 0) return 0;
   if (H % 4 != 0) return set_error("bb_embed_sum: H must be a multiple of 4");
+  if (!aligned16({word, pos, type0, out})) return set_error("bb_embed_sum: word / pos / type0 / out must be 16-byte aligned");
   const long long n = ntok * (H / 4);
   bb::launch_pdl(embed_sum_kernel, (unsigned)((n + 255) / 256), 256, 0, STREAM, ids, word, pos, type0, ntok, L, H, out);
   count_launch();
@@ -1162,6 +1181,7 @@ extern "C" int bb_embed_scatter_grad(const int64_t* ids, const float* dz, int64_
 extern "C" int bb_gather_rows_bf16(const void* in, const int64_t* idx, int64_t nout, int H, void* out, void* stream) {
   if (nout <= 0) return 0;
   if (H % 8 != 0) return set_error("bb_gather_rows_bf16: H must be a multiple of 8");
+  if (!aligned16({in, out})) return set_error("bb_gather_rows_bf16: in / out must be 16-byte aligned");
   const long long n = nout * (H / 8);
   ACT_T(bb::launch_pdl(gather_rows_bf16_kernel<T>, (unsigned)((n + 255) / 256), 256, 0, STREAM, (const T*)in, idx, nout, H, (T*)out));
   count_launch();

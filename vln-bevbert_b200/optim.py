@@ -63,7 +63,7 @@ class AdamW:
         self.m = self.v = None
         self._sumsq = None
         self._tables = {}       # gradient signature -> (MtTable, [flat index], shadow entries fully covered)
-        self.grad_norm = None   # 0-d device tensor of the last step (pre-clip total norm), when clipping is on
+        self.grad_norm = None   # device sum of squares of the last clipped step's gradients (total_grad_norm: its sqrt)
         self.last_sig = None
 
     # ------------------------------------------------------------------ state
@@ -174,7 +174,7 @@ class AdamW:
             for i in idx:
                 self.flat[i][1].grad = None
         self.last_sig = sig
-        return self.grad_norm
+        return self.total_grad_norm() if clip else None
 
     def advance(self, sig):
         """CUDA-graph replay of a captured step(): the graph re-uploads the pinned table and re-launches the kernels;
@@ -189,7 +189,7 @@ class AdamW:
 
     def total_grad_norm(self):
         """sqrt of the device-side sum of squares of the last clipped step (0-d tensor, no sync)."""
-        return None if self.grad_norm is None else self.grad_norm.sqrt()
+        return None if self.grad_norm is None else self.grad_norm.sqrt().reshape(())
 
     def zero_grad(self, set_to_none=True):
         for _, p in self.flat:
