@@ -54,6 +54,7 @@ class Runtime:
         self.feat_p = 0.0     # feature dropout requested by the pre-training wrapper (pretrain_cmt.py:102-106)
         self.calls = 0
         self._stream_id = None
+        self._training = False    # mode of the previous begin(): a train -> eval switch re-casts the shadows
 
     def begin(self, training: bool, seed=None, tag=None):
         self.calls += 1
@@ -70,6 +71,9 @@ class Runtime:
             SCRATCH.new_step(tag)
             if not self.wc.managed:     # a foreign optimizer may have stepped since the last forward (see WeightCache)
                 self.wc.refresh_all()
+        elif self._training and not self.wc.managed:
+            self.wc.refresh_all()       # first eval forward after training: the last optimizer step is not seen yet
+        self._training = training
         return self.ds
 
 
@@ -92,8 +96,11 @@ class WeightCache:
         update kernel and marks stale only the shadows it could not write (zero-padded tiny operands);
       * with any other optimizer `Runtime.begin(training=True)` advances the epoch at the
         start of every training forward, which re-casts all stacked / plain shadows in ONE multi-tensor launch
-        (`refresh_all`, ~1.1 GB of traffic = ~0.2 ms per step on this model);
-      * `p._version` is still compared, which covers `load_state_dict` / `copy_` in eval mode."""
+        (`refresh_all`, ~1.1 GB of traffic = ~0.2 ms per step on this model), and the first `begin(training=False)`
+        after a training forward does the same once, so validation after an optimizer step evaluates the new weights;
+      * `p._version` is still compared, which covers `load_state_dict` / `copy_` in eval mode.
+    An in-place update that bumps no version (`p.data.add_()`, torch's fused AdamW) made while the model stays in eval
+    mode is not seen: call `invalidate()` after it."""
 
     def __init__(self):
         self._c = {}
