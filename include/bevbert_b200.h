@@ -205,7 +205,8 @@ int bb_colsum_bf16(const void* x, int64_t rows, int N, int64_t ld, float* out, v
  * scores f32 (nbatch, H, nq, ld) already scaled; kmask f32 (nbatch, nk) additive (0 / -10000 / -inf) or NULL;
  * bias f32 (nbatch, nq, nk) additive, shared by heads (graph_sprels, vilmodel.py:391-392) or NULL.
  * probs bf16 (same layout); probs_drop bf16 = dropout(probs) when thresh != 0 (else may be NULL).
- * Columns [nk, ld) of the outputs are written as zeros. */
+ * Columns [nk, ld) of the outputs are written as zeros, and so is every column of a row whose keys are all -inf
+ * (as bb_flash_fwd gives), so that its dS and its share of dbias are 0. */
 int bb_softmax_fwd(const float* scores, const float* kmask, const float* bias, int nbatch, int H, int nq, int nk,
                    int ld, uint64_t seed, uint32_t thresh, float scale, void* probs, void* probs_drop, void* stream);
 /* dS = P * (dPd*keep*scale - sum_k(P * dPd*keep*scale)) * out_scale ; dP f32 (.., ld) wrt dropped probs;
@@ -273,7 +274,9 @@ int bb_softmax_xent(const float* logits, const int64_t* labels, int64_t rows, in
  * Bm = K (mode 0) or V (mode 1) likewise with nk rows.  P / Pd / Pin / dS are bf16 (B,H,nq,ldp).
  *   mode 0: P = softmax(alpha*A Bm^T + kmask + bias), Pd = dropout(P) (Pd may be NULL)
  *   mode 1: dS = Pin o (g - sum_k Pin g) * out_scale with g = dropout-mask(A Bm^T); dbias (B,nq,nk) f32 += unscaled
- * Same dropout counters as bb_softmax_fwd/bwd (vilmodel.py:117-127, 335-346).
+ * Same dropout counters as bb_softmax_fwd/bwd (vilmodel.py:117-127, 335-346); a row whose keys are all -inf gives
+ * P = Pd = 0.  bf16 only: fails while bb_set_act_f32(1) is on.  P / Pd / Pin / dS must be 4-byte aligned; B, H or
+ * nq <= 0 returns 0 without a launch.
  * ------------------------------------------------------------------------------------------- */
 typedef struct bb_attn_scores_args {
   const void* A; int64_t lda, a_s1, a_s2;

@@ -310,20 +310,33 @@ def colsum(x, N, out=None):
     return out
 
 
+def _softmax_keep(drop, nbatch, H, nq, nk, ld):
+    import drop_masks
+    return drop_masks.softmax_keep(drop[0], nbatch, H, nq, nk, ld, drop[1])
+
+
 def softmax_fwd(scores, kmask, bias, nbatch, H, nq, nk, ld, drop=(0, 0, 1.0)):
-    assert drop[1] == 0
+    """P (and its dropped copy) with zeros in the columns [nk, ld) and on rows whose keys are all -inf"""
     s = scores[..., :nk].clone()
     if kmask is not None:
         s = s + kmask.view(nbatch, 1, 1, nk)
     if bias is not None:
         s = s + bias.view(nbatch, 1, nq, nk)
     p = torch.zeros(nbatch, H, nq, ld, dtype=ACT)
-    p[..., :nk] = torch.softmax(s, -1)
-    return p, p
+    p32 = torch.nan_to_num(torch.softmax(s, -1), nan=0.0)
+    p[..., :nk] = p32
+    if not drop[1]:
+        return p, p
+    pd = torch.zeros_like(p)
+    keep = _softmax_keep(drop, nbatch, H, nq, nk, ld)
+    pd[..., :nk] = torch.where(keep, p32 * drop[2], torch.zeros_like(p32))
+    return p, pd
 
 
 def softmax_bwd(probs, dprobs, nbatch, H, nq, nk, ld, drop, out_scale, dbias=None):
     p, g = probs[..., :nk].to(F32), dprobs[..., :nk]
+    if drop[1]:
+        g = torch.where(_softmax_keep(drop, nbatch, H, nq, nk, ld), g * drop[2], torch.zeros_like(g))
     d = p * (g - (p * g).sum(-1, keepdim=True))
     ds = torch.zeros(nbatch, H, nq, ld, dtype=ACT)
     ds[..., :nk] = d * out_scale

@@ -358,7 +358,7 @@ def attn_core_fwd(st, q, ldq, k, ldk, v, ldv, B, H, nq, nk, dh, kmask, bias, dro
         ctx, lse = K.flash_fwd(q, k, v, B, H, nq, nk, ldq, ldk, ldv, kmask, bias, drop)
         st.update(lse=lse, fctx=ctx, geo=(B, H, nq, nk, dh, ldp), adrop=drop, amask=(kmask, bias))
         return ctx.view(B * nq, H * dh)
-    if nk <= K.FUSED_SCORES_MAX_KEYS and dh == 64:
+    if K._fused_scores(nk, dh):
         P, Pd = K.attn_scores_fwd(q, ldq, k, ldk, B, H, nq, nk, dh, ldp, kmask, bias, drop)
     else:
         S = _empty((B, H, nq, ldp), q, torch.float32)
@@ -386,7 +386,7 @@ def attn_core_bwd(st, dctx, q, ldq, k, ldk, v, ldv, dq, lddq, dk, lddk, dv, lddv
     # dV = Pd^T dctx
     K.gemm(Pd, dctx, dv, nk, dh, nq, lda=ldp, ldb=HD, ldd=lddv, a_mn=True, b_mn=True, nb1=H, nb2=B,
            a_s=(nq * ldp, H * nq * ldp), b_s=(dh, nq * HD), d_s=(dh, nk * lddv))
-    if nk <= K.FUSED_SCORES_MAX_KEYS and dh == 64:
+    if K._fused_scores(nk, dh):
         dS = K.attn_scores_bwd(dctx, HD, v, ldv, P, B, H, nq, nk, dh, ldp, drop, dbias)
     else:
         # dPd = dctx V^T

@@ -23,6 +23,8 @@
 
 namespace bb {
 
+bool act_f32();   // gemm_f32.cu: fp32-activation verification mode (bb_set_act_f32)
+
 constexpr int AS_THREADS = 288;            // warps 0..7: two consumer warpgroups (64 query rows each), warp 8: TMA
 constexpr int AS_Q_BYTES = 128 * 64 * 2;   // 16 KB
 constexpr int AS_K_BYTES = 512 * 64 * 2;   // 64 KB
@@ -181,7 +183,11 @@ attn_scores_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       for (int hh = 0; hh < 2; ++hh) {
         m[hh] = quad_max_f(mx[hh]);
         const float part = mx[hh] > -INFINITY ? sum[hh] * __expf(mx[hh] - m[hh]) : 0.0f;
-        inv[hh] = 1.0f / quad_sum_f(part);   // all keys masked with -inf: 1/0 -> inf, probabilities NaN like torch
+        const float tot = quad_sum_f(part);
+        // all keys masked with -inf: P = Pd = 0 (exp(-inf - 0) * 0), as bb_softmax_fwd and the flash cores give, so
+        // that dS and the graph-bias gradient of the row are 0 as well
+        inv[hh] = tot > 0.0f ? 1.0f / tot : 0.0f;
+        if (m[hh] == -INFINITY) m[hh] = 0.0f;
       }
       // pass B: probabilities (and their dropped copy)
       for (int c = 0; c < nkb_out; ++c) {
@@ -316,10 +322,17 @@ extern "C" int bb_attn_scores(const bb_attn_scores_args* a, void* stream_) {
   using namespace bb;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!a || !a->A || !a->Bm) return set_error("bb_attn_scores: null argument");
+  if (act_f32())
+    return set_error("bb_attn_scores: bf16 operands and outputs only; the fp32 verification mode (bb_set_act_f32) runs "
+                     "the unfused GEMM + bb_softmax_fwd/bwd sequence");
+  if (a->B <= 0 || a->H <= 0 || a->nq <= 0) return 0;
   if (a->nk < 1 || a->nk > 512) return set_error("bb_attn_scores: needs 1 <= nk <= 512 keys per row");
   if (a->ldp % 8 != 0 || a->ldp < a->nk) return set_error("bb_attn_scores: ldp must be a multiple of 8 and >= nk");
   if (a->mode == 0 && !a->P) return set_error("bb_attn_scores: mode 0 needs P");
   if (a->mode == 1 && (!a->Pin || !a->dS)) return set_error("bb_attn_scores: mode 1 needs Pin and dS");
+  // P / Pd / Pin / dS are stored and read as bf16 pairs
+  for (const void* t : {(const void*)a->P, (const void*)a->Pd, a->Pin, (const void*)a->dS})
+    if (reinterpret_cast<uintptr_t>(t) & 3) return set_error("bb_attn_scores: P, Pd, Pin and dS must be 4-byte aligned");
   if (a->mode == 1 && a->dbias && det_mode() == 1)
     return set_error("bb_attn_scores: the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient adds with fp32 atomics "
                      "and has no deterministic implementation");

@@ -27,6 +27,9 @@ static inline int fused_max_keys() {
   }
   return v;
 }
+bool act_f32();   // gemm_f32.cu: fp32-activation verification mode (bb_set_act_f32)
+// fused scores + softmax (attn_scores.cu) instead of the GEMM -> bb_softmax pair: bf16 only, head dim 64
+static inline bool fused_scores(int nk, int dh) { return nk <= fused_max_keys() && dh == 64 && !act_f32(); }
 static inline int round8(int n) { return (n + 7) / 8 * 8; }
 // fused attention core (attn_flash.cu) for head dim 64; BB_FLASH=0 selects the unfused GEMM + softmax sequence
 static inline bool flash_on(const bb_attn_desc* d) {
@@ -178,7 +181,7 @@ static int attn_core_fwd(const bb_attn_desc* d, const AttnLayout& L, const void*
     return bb_flash_fwd(&f, stream);
   }
   bb_gemm_args g;
-  if (nk <= fused_max_keys() && dh == 64) {
+  if (fused_scores(nk, dh)) {
     bb_attn_scores_args s;
     memset(&s, 0, sizeof(s));
     s.A = q; s.lda = ldq; s.a_s1 = dh; s.a_s2 = (int64_t)nq * ldq;
@@ -235,7 +238,7 @@ static int attn_core_bwd(const bb_attn_desc* d, const AttnLayout& L, const void*
   g.lda = ldp; g.a_s1 = ps1; g.a_s2 = ps2; g.ldb = HD; g.b_s1 = dh; g.b_s2 = (int64_t)nq * HD;
   g.ldd = lddv; g.d_s1 = dh; g.d_s2 = (int64_t)nk * lddv; g.split_k = 1; g.alpha = 1.0f; g.drop_scale = 1.0f;
   TRY(bb_gemm_bf16(&g, stream));
-  if (nk <= fused_max_keys() && dh == 64) {
+  if (fused_scores(nk, dh)) {
     bb_attn_scores_args s;
     memset(&s, 0, sizeof(s));
     s.A = dctx; s.lda = HD; s.a_s1 = dh; s.a_s2 = (int64_t)nq * HD;

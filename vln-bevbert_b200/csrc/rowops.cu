@@ -634,6 +634,8 @@ softmax_fwd_kernel(const float* __restrict__ scores, const float* __restrict__ k
     mx = fmaxf(mx, t);
   }
   mx = warp_max(mx);
+  // every key masked with -inf: exp(-inf - 0) = 0 and P = Pd = 0, as the flash cores give, instead of -inf - -inf = NaN
+  if (mx == -INFINITY) mx = 0.f;
   float sum = 0.f;
 #pragma unroll
   for (int e = 0; e < MAXE; ++e) {
@@ -643,7 +645,7 @@ softmax_fwd_kernel(const float* __restrict__ scores, const float* __restrict__ k
     sum += ex;
   }
   sum = warp_sum(sum);
-  const float inv = 1.0f / sum;
+  const float inv = sum > 0.f ? 1.0f / sum : 0.f;
   T* p = probs + row * ld;
   T* pd = probs_drop ? probs_drop + row * ld : nullptr;
 #pragma unroll

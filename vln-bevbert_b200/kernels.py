@@ -257,8 +257,7 @@ def sublayer_fwd(d):
 
 def sublayer_bwd(d):
     lib = _lib.load()
-    if (isinstance(d, _lib.AttnDesc) and d.want_dbias and not FLASH and d.Hd // d.heads == 64
-            and d.nk <= FUSED_SCORES_MAX_KEYS):
+    if isinstance(d, _lib.AttnDesc) and d.want_dbias and not FLASH and _fused_scores(d.nk, d.Hd // d.heads):
         _nondeterministic("the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient")
     fn = {_lib.AttnDesc: lib.bb_attn_bwd, _lib.FfnDesc: lib.bb_ffn_bwd, _lib.PanoDesc: lib.bb_pano_bwd}[type(d)]
     _lib.check(fn(C.byref(d), _stream()), "bb_sublayer_bwd")
@@ -267,9 +266,17 @@ def sublayer_bwd(d):
 FUSED_SCORES_MAX_KEYS = min(512, int(__import__('os').environ.get('BB_FUSED_SCORES_MAX', '0')))
 
 
+def _fused_scores(nk, dh):
+    """the unfused attention path forms P / dS with bb_attn_scores (the BB_FUSED_SCORES_MAX experiment) instead of a
+    GEMM and bb_softmax_fwd/bwd: bf16 operands only, so never in the fp32 verification arm"""
+    return not _FP32_ARM and dh == 64 and nk <= FUSED_SCORES_MAX_KEYS
+
+
 def attn_scores_fwd(q, ldq, k, ldk, B, H, nq, nk, dh, ldp, kmask, bias, drop):
     """fused P = softmax(Q K^T / sqrt(dh) + kmask + bias) (+ dropped copy): -> (P, Pd) bf16 (B,H,nq,ldp)."""
     lib = _lib.load()
+    _req(q, BF16, "q")
+    _req(k, BF16, "k")
     a = _lib.AttnScoresArgs()
     a.A, a.lda, a.a_s1, a.a_s2 = q.data_ptr(), ldq, dh, nq * ldq
     a.Bm, a.ldb, a.b_s1, a.b_s2 = k.data_ptr(), ldk, dh, nk * ldk
@@ -277,8 +284,8 @@ def attn_scores_fwd(q, ldq, k, ldk, B, H, nq, nk, dh, ldp, kmask, bias, drop):
     a.alpha = 1.0 / (dh ** 0.5)
     a.kmask, a.bias = _p(kmask), _p(bias)
     a.seed, a.thresh, a.scale = drop
-    P = torch.empty(B, H, nq, ldp, dtype=act_dtype(), device=q.device)
-    Pd = torch.empty(B, H, nq, ldp, dtype=act_dtype(), device=q.device) if drop[1] else None
+    P = torch.empty(B, H, nq, ldp, dtype=BF16, device=q.device)
+    Pd = torch.empty(B, H, nq, ldp, dtype=BF16, device=q.device) if drop[1] else None
     a.P, a.Pd = P.data_ptr(), _p(Pd)
     _lib.check(lib.bb_attn_scores(C.byref(a), _stream()), "bb_attn_scores")
     return P, (Pd if Pd is not None else P)
@@ -287,6 +294,8 @@ def attn_scores_fwd(q, ldq, k, ldk, B, H, nq, nk, dh, ldp, kmask, bias, drop):
 def attn_scores_bwd(dctx, ldd, v, ldv, P, B, H, nq, nk, dh, ldp, drop, dbias=None):
     """fused dS = P o (g - sum P g) / sqrt(dh), g = dropout-mask(dctx V^T): -> dS bf16 (B,H,nq,ldp)."""
     lib = _lib.load()
+    for t, n in ((dctx, "dctx"), (v, "v"), (P, "P")):
+        _req(t, BF16, n)
     if dbias is not None:
         _nondeterministic("the fused-scores (BB_FUSED_SCORES_MAX) graph-bias gradient")
     a = _lib.AttnScoresArgs()
@@ -295,7 +304,7 @@ def attn_scores_bwd(dctx, ldd, v, ldv, P, B, H, nq, nk, dh, ldp, drop, dbias=Non
     a.B, a.H, a.nq, a.nk, a.ldp, a.mode = B, H, nq, nk, ldp, 1
     a.alpha, a.out_scale = 1.0, 1.0 / (dh ** 0.5)
     a.seed, a.thresh, a.scale = drop
-    dS = torch.empty(B, H, nq, ldp, dtype=act_dtype(), device=dctx.device)
+    dS = torch.empty(B, H, nq, ldp, dtype=BF16, device=dctx.device)
     a.Pin, a.dS, a.dbias = P.data_ptr(), dS.data_ptr(), _p(dbias)
     _lib.check(lib.bb_attn_scores(C.byref(a), _stream()), "bb_attn_scores")
     return dS
