@@ -172,7 +172,7 @@ int bb_bev_splat_nodes(const bb_bev_node* nodes, int n_nodes, const int32_t* sam
 /* ---------------------------------------------------------------------------------------------
  * Row kernels (coalesced, vectorised, warp reductions; fp32 math, bf16 storage).
  * Every row-matrix and vector pointer of the entry points below that read or write 16-byte vectors (LayerNorm forward /
- * backward, bb_add_rows, bb_gather_rows_bf16, bb_segment_wsum / _bwd, bb_embed_sum, bb_colsum_bf16 when ld % 8 == 0,
+ * backward, bb_add_rows, bb_add_rows3, bb_gather_rows_bf16, bb_segment_wsum / _bwd, bb_embed_sum, bb_colsum_bf16 when ld % 8 == 0,
  * the casts, bb_scatter_rows_sorted) must be 16-byte aligned; a misaligned one is rejected with an error, nothing runs.
  * ------------------------------------------------------------------------------------------- */
 /* f32 -> bf16 cast with optional inverted dropout (nn.Dropout on inputs, pretrain_cmt.py:102-106).
@@ -244,6 +244,14 @@ int bb_dropout_bf16(const void* src, void* dst, int64_t n, uint64_t seed, uint32
  * (embedding sums of vilmodel.py:521-524, 590-592, 675-677). b/table/idx/vec may be NULL. */
 int bb_add_rows(const void* a, const void* b, const float* table, const int64_t* idx, const float* vec, int64_t rows,
                 int H, void* out, void* stream);
+/* out[r,:] = ((a[r,:] + b[r,:]) + c[r,:]) (+ table[idx[r],:]) (+ vec[:]), summed in that order in fp32; a, b, c, out
+ * activations with row strides lda / ldb / ldc / ldo (elements, each >= H and a multiple of 8); table, vec f32; idx
+ * int64.  The VLN-CE view embedding: image + depth + location terms, nav-type row and type vector
+ * (bevbert_ce/pretrain/pretrain_src/model/vilmodel.py:506-533).  table/idx/vec may be NULL; a, b, c, out may not.
+ * Only columns [0, H) of each row are read or written.  Its backward hands the output gradient to a, b and c unchanged
+ * and reduces the table / vec gradients with bb_scatter_add_rows (or bb_scatter_rows_sorted) and bb_colsum_bf16. */
+int bb_add_rows3(const void* a, int64_t lda, const void* b, int64_t ldb, const void* c, int64_t ldc, const float* table,
+                 const int64_t* idx, const float* vec, int64_t rows, int H, void* out, int64_t ldo, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

@@ -137,6 +137,8 @@ _SIGNATURES = {
     "bb_dropout_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_u64, c_u32, c_float, c_void_p]),
     "bb_act_bwd_bf16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_i64, c_void_p]),
     "bb_add_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
+    "bb_add_rows3": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64,
+                             c_int, c_void_p, c_i64, c_void_p]),
     "bb_scale_rows_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p]),
     "bb_segment_wsum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_segment_wsum_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),

@@ -931,6 +931,27 @@ class AddRowsImpl:
         return [g, g if st["has_b"] else None, None], [dt, dv]
 
 
+class AddRows3Impl(AddRowsImpl):
+    """out = ((a + b) + c) (+ table[idx]) (+ vec_src[vec_row]) in one bb_add_rows3 launch; a,b,c activations (rows,Hd).
+    inputs (a, b, c, idx | None); params (table | None, vec_src | None).  Backward as AddRowsImpl: the output gradient
+    goes to a, b and c unchanged."""
+
+    def fwd(self, st, inputs, p):
+        a, b, c, idx = inputs
+        table, vsrc = p
+        Hd = a.shape[-1]
+        i2 = idx.reshape(-1).contiguous() if idx is not None else None
+        vec = vsrc.detach()[self.vec_row].contiguous() if vsrc is not None else None
+        out = K.add_rows(a.reshape(-1, Hd), b.reshape(-1, Hd), table.detach() if table is not None else None, i2, vec,
+                         c=c.reshape(-1, Hd))
+        st.update(idx=i2, shape=a.shape, has_b=True)
+        return out.view(a.shape)
+
+    def bwd(self, st, gouts, p):
+        (g, _, _), dp = super().bwd(st, gouts, p)
+        return [g, g, g, None], dp
+
+
 class SegmentSumImpl:
     """out[s] = sum_e w[e] * src[idx[e]] over CSR segments (gmap node features, vilmodel.py:632-666).
     inputs (src (rows,Hd), seg_off int32, idx int32, w f32); no params."""

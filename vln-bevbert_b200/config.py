@@ -13,6 +13,14 @@ R2R_DEFAULTS = dict(
     pretrain_tasks=["mlm", "sap", "masksem"], sem_pred_token="cattn",
 )
 
+# VLN-CE pre-training (bevbert_ce/pretrain/run_pt/r2r_model_config_dep.json; tasks of r2r_pretrain_habitat.json):
+# 512-d CLIP view features, 128-d depth features, 4 angle columns, no objects, an 11 x 11 BEV at 1 m
+CE_DEFAULTS = dict(R2R_DEFAULTS, image_feat_size=512, depth_feat_size=128, image_prob_size=1000, bev_dim=11, bev_res=1.0,
+                   pretrain_tasks=["mlm", "sap"])
+# a 2/1/2-layer CE model with dropout off: the parity tests' and smoke runs' size
+CE_SMALL = dict(num_l_layers=2, num_x_layers=2, num_pano_layers=1, vocab_size=3000, hidden_dropout_prob=0.0,
+                attention_probs_dropout_prob=0.0, feat_dropout=0.0)
+
 
 def make_config(**overrides):
     """Returns a transformers.PretrainedConfig when transformers is importable (what the reference's
@@ -27,3 +35,12 @@ def make_config(**overrides):
         return cfg
     except Exception:  # pragma: no cover
         return SimpleNamespace(**vals)
+
+
+def make_ce_config(small=False, **overrides):
+    """make_config for the VLN-CE model (model/ce_pretrain.py); `small` applies CE_SMALL before `overrides`."""
+    vals = dict(CE_DEFAULTS)
+    if small:
+        vals.update(CE_SMALL)
+    vals.update(overrides)
+    return make_config(**vals)

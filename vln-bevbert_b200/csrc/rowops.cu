@@ -198,6 +198,40 @@ __global__ void add_rows_kernel(const T* __restrict__ a, const T* __restrict__ b
   }
   store8(out + r * H + c, v);
 }
+// out = ((a + b) + c) (+ table[idx[r]]) (+ vec), each row operand with its own row stride: the VLN-CE view embedding
+// (image + depth + location terms, bevbert_ce/pretrain/pretrain_src/model/vilmodel.py:506-533) in one pass
+template <typename T>
+__global__ void add_rows3_kernel(const T* __restrict__ a, long long lda, const T* __restrict__ b, long long ldb,
+                                 const T* __restrict__ c3, long long ldc, const float* __restrict__ table,
+                                 const int64_t* __restrict__ idx, const float* __restrict__ vec, long long rows, int H,
+                                 T* __restrict__ out, long long ldo) {
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  const int h8 = H / 8;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= rows * h8) return;
+  const long long r = i / h8;
+  const int c = (i % h8) * 8;
+  float v[8], t[8];
+  load8(a + r * lda + c, v);
+  load8(b + r * ldb + c, t);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] += t[j];
+  load8(c3 + r * ldc + c, t);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] += t[j];
+  if (table) {
+    load8(table + idx[r] * H + c, t);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] += t[j];
+  }
+  if (vec) {
+    load8(vec + c, t);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] += t[j];
+  }
+  store8(out + r * ldo + c, v);
+}
 template <typename T>
 __global__ void scale_rows_bf16_kernel(T* __restrict__ x, const float* __restrict__ g, long long rows, long long ld) {
   bb::pdl_wait();
@@ -958,6 +992,24 @@ extern "C" int bb_add_rows(const void* a, const void* b, const float* table, con
                                                                    rows, H, (T*)out));
   count_launch();
   return check_launch("add_rows_kernel");
+}
+extern "C" int bb_add_rows3(const void* a, int64_t lda, const void* b, int64_t ldb, const void* c, int64_t ldc,
+                            const float* table, const int64_t* idx, const float* vec, int64_t rows, int H, void* out,
+                            int64_t ldo, void* stream) {
+  if (rows <= 0) return 0;
+  if (H <= 0 || H % 8 != 0) return set_error("bb_add_rows3: H must be a positive multiple of 8");
+  if (!a || !b || !c || !out) return set_error("bb_add_rows3: a / b / c / out must not be NULL");
+  if (table && !idx) return set_error("bb_add_rows3: table needs idx");
+  for (int64_t ld : {lda, ldb, ldc, ldo})
+    if (ld < H || ld % 8 != 0) return set_error("bb_add_rows3: every row stride must be >= H and a multiple of 8");
+  if (!aligned16({a, b, c, table, vec, out}))
+    return set_error("bb_add_rows3: a / b / c / table / vec / out must be 16-byte aligned");
+  const long long n = rows * (H / 8);
+  ACT_T(bb::launch_pdl(add_rows3_kernel<T>, (unsigned)((n + 255) / 256), 256, 0, STREAM, (const T*)a, (long long)lda,
+                       (const T*)b, (long long)ldb, (const T*)c, (long long)ldc, table, idx, vec, (long long)rows, H,
+                       (T*)out, (long long)ldo));
+  count_launch();
+  return check_launch("add_rows3_kernel");
 }
 extern "C" int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream) {
   if (rows <= 0) return 0;

@@ -591,13 +591,27 @@ def relu_bwd(dy, post):
     return _act_bwd(dy, post, 2)
 
 
-def add_rows(a, b=None, table=None, idx=None, vec=None):
-    """a (+ b) (+ table[idx]) (+ vec) over bf16 (rows,H)."""
+def add_rows(a, b=None, table=None, idx=None, vec=None, c=None, out=None):
+    """a (+ b) (+ table[idx]) (+ vec) over activation rows (rows,H) (bb_add_rows).  With a third row operand `c` (and
+    `b`): ((a + b) + c) (+ table[idx]) (+ vec) in one bb_add_rows3 launch, where a / b / c / `out` may be row-strided
+    views with unit column stride; `out` (only with `c`) is the (rows,H) destination, else a new contiguous tensor."""
     lib = _lib.load()
     rows, H = a.shape
-    out = torch.empty(rows, H, dtype=act_dtype(), device=a.device)
-    _lib.check(lib.bb_add_rows(a.data_ptr(), _p(b), _p(table), _p(idx), _p(vec), rows, H, out.data_ptr(), _stream()),
-               "bb_add_rows")
+    if c is None:
+        if out is not None:
+            raise ValueError("add_rows: `out` is taken only with the third row operand `c` (bb_add_rows3)")
+        out = torch.empty(rows, H, dtype=act_dtype(), device=a.device)
+        _lib.check(lib.bb_add_rows(a.data_ptr(), _p(b), _p(table), _p(idx), _p(vec), rows, H, out.data_ptr(),
+                                   _stream()), "bb_add_rows")
+        return out
+    if out is None:
+        out = torch.empty(rows, H, dtype=act_dtype(), device=a.device)
+    for t in (a, b, c, out):
+        if t is None or t.dim() != 2 or t.shape[0] != rows or t.shape[1] != H or t.stride(1) != 1:
+            raise ValueError("add_rows with c: a, b, c and out must be (rows, H) matrices with unit column stride")
+    _lib.check(lib.bb_add_rows3(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), c.data_ptr(), c.stride(0),
+                                _p(table), _p(idx), _p(vec), rows, H, out.data_ptr(), out.stride(0), _stream()),
+               "bb_add_rows3")
     return out
 
 

@@ -98,7 +98,7 @@ class PreparedList(list):
     host_mlm = None
 
 
-WIRE_KEYS = ("rgbs", "traj_view_img_fts", "traj_obj_img_fts")
+WIRE_KEYS = ("rgbs", "traj_view_img_fts", "traj_view_dep_fts", "traj_obj_img_fts")
 
 
 def prepare_batch(batch, wire_dtype=None):

@@ -162,6 +162,10 @@ class GlocalTextPathCMTPreTraining(PreTrainedBase):
             txt_ids, txt_lens, traj_view_img_fts, traj_obj_img_fts, traj_loc_fts, traj_nav_types, traj_step_lens,
             traj_vp_view_lens, traj_vp_obj_lens, traj_vpids, traj_cand_vpids, gmap_lens, gmap_step_ids, gmap_pos_fts,
             gmap_pair_dists, gmap_vpids, bev_fts, bev_pos_fts, bev_masks, bev_nav_masks)
+        return self._mlm_head(txt_embeds, gmap_vpids, txt_labels, compute_loss)
+
+    def _mlm_head(self, txt_embeds, gmap_vpids, txt_labels, compute_loss):
+        """pretrain_cmt.py:217-227: MLM scores / loss of the masked text rows."""
         impl = Bk.MLMLossImpl(self.rt, self.mlm_head.eps, compute_loss)
         pre = getattr(gmap_vpids, "host_mlm", None)      # ops.prepare_batch(): masked rows listed at collate time
         if pre is not None and pre[0] == tuple(txt_labels.shape):
@@ -191,11 +195,17 @@ class GlocalTextPathCMTPreTraining(PreTrainedBase):
                     traj_step_lens, traj_vp_view_lens, traj_vp_obj_lens, traj_vpids, traj_cand_vpids, gmap_lens,
                     gmap_step_ids, gmap_pos_fts, gmap_pair_dists, gmap_vpids, gmap_visited_masks, bev_fts, bev_pos_fts,
                     bev_masks, bev_nav_masks, bev_cand_idxs, global_act_labels, local_act_labels, compute_loss):
-        B = txt_ids.size(0)
         gmap_embeds, bev_embeds, _, _ = self.bert(
             txt_ids, txt_lens, traj_view_img_fts, traj_obj_img_fts, traj_loc_fts, traj_nav_types, traj_step_lens,
             traj_vp_view_lens, traj_vp_obj_lens, traj_vpids, traj_cand_vpids, gmap_lens, gmap_step_ids, gmap_pos_fts,
             gmap_pair_dists, gmap_vpids, bev_fts, bev_pos_fts, bev_masks, bev_nav_masks)
+        return self._sap_head(gmap_embeds, bev_embeds, traj_cand_vpids, gmap_lens, gmap_vpids, gmap_visited_masks,
+                              bev_nav_masks, bev_cand_idxs, global_act_labels, local_act_labels, compute_loss)
+
+    def _sap_head(self, gmap_embeds, bev_embeds, traj_cand_vpids, gmap_lens, gmap_vpids, gmap_visited_masks,
+                  bev_nav_masks, bev_cand_idxs, global_act_labels, local_act_labels, compute_loss):
+        """pretrain_cmt.py:322-366: global / local / fused action logits and their losses."""
+        B = gmap_embeds.shape[0]
         G, Kc = gmap_embeds.shape[1], bev_cand_idxs.shape[1]
         n = self.config.bev_dim * self.config.bev_dim
         dev = gmap_embeds.device

@@ -99,10 +99,13 @@ class SynthConfig:
     obj_prob_size: int = 1000
     depth_zero_frac: float = 0.05
     ragged_txt: bool = False     # variable instruction lengths (txt_lens < txt_len)
+    depth_feat_size: int = 0     # >0: VLN-CE batch (traj_view_dep_fts, 4 location columns, no semantic labels)
 
 
 def make_batch(cfg: SynthConfig, seed: int = 1234, task: str = "sap") -> dict:
-    """One collated batch (CPU tensors + host lists) for `task` in {mlm, sap, masksem, sem, mrc, og}."""
+    """One collated batch (CPU tensors + host lists) for `task` in {mlm, sap, masksem, sem, mrc, og}.  With
+    cfg.depth_feat_size > 0 it is laid out as the VLN-CE collate gives it (bevbert_ce/pretrain/pretrain_src/data): depth
+    features per view, location features of 4 angle columns and no `sems`; everything else is drawn as for R2R."""
     B, L, D = cfg.batch_size, cfg.txt_len, cfg.bev_dim
     ncell = D * D
     s = [0]
@@ -325,7 +328,19 @@ def make_batch(cfg: SynthConfig, seed: int = 1234, task: str = "sap") -> dict:
             lab = det_randint((B,), seed, stream(), 0, 1 << 20)
             batch["obj_labels"] = torch.tensor(
                 [int(lab[i]) % last_obj[i] if last_obj[i] > 0 else -100 for i in range(B)], dtype=torch.int64)
+    if cfg.depth_feat_size > 0:
+        # drawn last, so that every other tensor matches the R2R batch of the same seed
+        batch["traj_view_dep_fts"] = det_uniform((sumP, V, cfg.depth_feat_size), seed, stream(), -1.7320508, 1.7320508)
+        batch["traj_loc_fts"] = batch["traj_loc_fts"][:, :, :4].contiguous()
+        del batch["sems"]
     return batch
+
+
+def ce_synth_config(**kw) -> SynthConfig:
+    """SynthConfig of a VLN-CE batch: 512-d view and 128-d depth features, nav types {0, 1}, an 11 x 11 BEV at 1 m."""
+    d = dict(image_feat_size=512, depth_feat_size=128, bev_dim=11, bev_res=1.0)
+    d.update(kw)
+    return SynthConfig(**d)
 
 
 def batch_to(batch: dict, device, non_blocking: bool = False) -> dict:
@@ -363,8 +378,8 @@ def det_init_(model, seed: int = 0, std: float = 0.02):
     return model
 
 
-_PANO_KEYS = ("traj_view_img_fts", "traj_obj_img_fts", "traj_vp_obj_lens", "traj_loc_fts", "traj_nav_types",
-              "traj_vp_view_lens")
+_PANO_KEYS = ("traj_view_img_fts", "traj_view_dep_fts", "traj_obj_img_fts", "traj_vp_obj_lens", "traj_loc_fts",
+              "traj_nav_types", "traj_vp_view_lens")
 
 
 def split_batch(batch: dict, parts: int):
