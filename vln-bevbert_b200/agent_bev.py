@@ -11,7 +11,13 @@ agent's own methods (`_map_cand_to_bev`, `GraphMap.get_pos_fts`, `graph.path`, `
 Install on an agent once it is built:
 
     agent._nav_bev_variable = types.MethodType(nav_bev_variable, agent)
+
+`ce_nav_bev_variable(trainer, cur_vp, cur_pos, cur_ori)` does the same for the VLN-CE trainer's `_nav_bev_variable`
+(bevbert_ce/vlnce_baselines/ss_trainer_BEV.py:477-532); see its docstring.
 """
+import importlib
+import sys
+
 import numpy as np
 import torch
 
@@ -20,22 +26,29 @@ from . import bev_nodes
 Y_CLIP = 0.5    # height clip of the agents' project_bev (map_nav_src/models/bev_utils.py:398)
 
 
-def gathered_nodes(gmap, vp, order):
+def gathered_nodes(gmap, vp, order, path=None):
     """The viewpoints whose clouds `GraphMap.gather_node_pc(vp, order)` concatenates, in its order: the node alone at
-    order 0, otherwise every node with a cloud, in insertion order of `node_pc`, at most `order` graph hops from vp."""
+    order 0, otherwise every node with a cloud, in insertion order of `node_pc`, at most `order` graph hops from vp.
+    `path(vp, c)`: the shortest path the graph map keeps (default `gmap.graph.path`, the discrete agents')."""
     if order == 0:
         return [vp]
-    return [c for c in gmap.node_pc if len(gmap.graph.path(vp, c)) <= order]
+    path = path or gmap.graph.path
+    return [c for c in gmap.node_pc if len(path(vp, c)) <= order]
 
 
 def ego_frames(obs):
     """World -> ego transform of each sample, float32: S (B,3) = (x, z, -y) of the agent's position and T (B,4,4) a
     rotation about the vertical axis by the heading, built in float64 and rounded to float32 like the agents'
     matrices (agent.py:150-159)."""
-    h = np.array([o["heading"] for o in obs], dtype=np.float64)
-    c, s = np.cos(h), np.sin(h)
     S = np.array([[o["position"][0], o["position"][2], -o["position"][1]] for o in obs], dtype=np.float64)
-    T = np.zeros((len(obs), 4, 4), dtype=np.float64)
+    return heading_frames(S, np.array([o["heading"] for o in obs], dtype=np.float64))
+
+
+def heading_frames(S, h):
+    """(S, T) float32 from float64 positions S (B,3) and headings h (B,): T rotates about the vertical axis by h
+    (transfrom3D at zero elevation and translation, bev_utils.py:7-37 of both trees)."""
+    c, s = np.cos(h), np.sin(h)
+    T = np.zeros((len(h), 4, 4), dtype=np.float64)
     T[:, 0, 0], T[:, 0, 2] = c, s
     T[:, 1, 1] = 1.0
     T[:, 2, 0], T[:, 2, 2] = -s, c
@@ -73,6 +86,73 @@ def nav_bev_variable(agent, obs, gmaps):
     return {
         "bev_fts": bev_fts,
         "bev_pos_fts": torch.cat([gpos.expand(-1, D * D, -1), agent.bev_pos.reshape(B, -1, 3)], -1),
+        "bev_masks": torch.ones(B, D * D, dtype=torch.bool, device=dev),
+        "bev_nav_masks": torch.from_numpy(nav_masks).to(dev),
+        "bev_cand_idxs": bev_cand_idxs,
+        "bev_cand_vpids": cand_vpids,
+    }
+
+
+def _trainer_heading_fn(trainer):
+    """The `heading_from_quaternion` the trainer's own code uses: the one imported by the module of its class or of the
+    nearest base class (ss_trainer_BEV.py:61), else graph_utils' (where ss_trainer_BEV takes it from)."""
+    for cls in type(trainer).__mro__:
+        fn = getattr(sys.modules.get(cls.__module__), "heading_from_quaternion", None)
+        if fn is not None:
+            return fn
+    return importlib.import_module("vlnce_baselines.models.graph_utils").heading_from_quaternion
+
+
+def ce_nav_bev_variable(trainer, cur_vp, cur_pos, cur_ori):
+    """Drop-in for the VLN-CE trainer's `_nav_bev_variable(cur_vp, cur_pos, cur_ori)` (ss_trainer_BEV.py:477-532),
+    same dict.  The clouds of `GraphMap.gather_node_pc(vp, order=1)` (graph_utils.py:332-346: the nodes with a cloud
+    whose shortest path from vp has at most one node, i.e. vp itself) are transformed to each sample's ego frame and
+    pooled into the `trainer.bev_dim`-square map at `trainer.bev_res` by one `bb_bev_splat_nodes` launch, instead of
+    `pad_sequence` + `splat` (:413-463) + `PointCloud.project_bev`.  The ego frame is `splat`'s: S = (x, y, z) of the
+    position and T `transfrom3D` of heading -heading_from_quaternion(orientation), with the trainer's own
+    `heading_from_quaternion` (`_trainer_heading_fn`); like transfrom3D, T is built in float64 and rounded to float32.
+    The node clouds must be float32 points (the kernel transforms them in fp32, in a fixed order).  Candidates
+    (`GraphMap.get_neighbors`, the trainer's `_discretize_polar_relpos`) and the global position feature
+    (`GraphMap.get_pos_fts` towards the start node '0') come from the trainer's own objects.  `bev_masks` is all True,
+    as `splat` returns it without VIDEO_OPTION; `bev_cand_idxs` stays on the host, as the trainer's does (:511).
+
+    Install on the trainer once it is built:
+
+        trainer._nav_bev_variable = types.MethodType(ce_nav_bev_variable, trainer)
+    """
+    heading_from_quaternion = _trainer_heading_fn(trainer)
+    gmaps, D = trainer.gmaps, trainer.bev_dim
+    B = len(gmaps)
+    clouds = [[tuple(gm.node_pc[c]) for c in gathered_nodes(gm, vp, 1, lambda a, b, gm=gm: gm.shortest_path[a][b])]
+              for gm, vp in zip(gmaps, cur_vp)]
+    dev = trainer.bev_pos.device
+
+    nav_masks = np.zeros((B, D * D), dtype=bool)
+    cand_idxs, cand_vpids, gpos = [], [], []
+    for i, gm in enumerate(gmaps):
+        vps, relpos = gm.get_neighbors(cur_vp[i], cur_pos[i], cur_ori[i])
+        xy = trainer._discretize_polar_relpos(relpos)
+        idx = xy[:, 1] * D + xy[:, 0]
+        nav_masks[i, idx] = True
+        cand_idxs.append(idx)
+        cand_vpids.append(vps)
+        gpos.append(gm.get_pos_fts(cur_vp[i], cur_pos[i], cur_ori[i], ["0"]))       # '0' is the start node
+
+    S = np.array([[p[0], p[1], p[2]] for p in cur_pos], dtype=np.float64)
+    S, T = heading_frames(S, np.array([-heading_from_quaternion(o) for o in cur_ori], dtype=np.float64))
+    frames = torch.from_numpy(np.concatenate([S.ravel(), T.ravel()])).to(dev)     # one upload for both
+    bev_fts, _ = bev_nodes.bev_splat_nodes(clouds, frames[:3 * B].view(B, 3), frames[3 * B:].view(B, 4, 4), D,
+                                           trainer.bev_res, Y_CLIP, C=768)
+
+    L = max(len(c) for c in cand_idxs)
+    bev_cand_idxs = torch.zeros(B, L, dtype=torch.from_numpy(cand_idxs[0]).dtype)
+    for i, c in enumerate(cand_idxs):
+        bev_cand_idxs[i, :len(c)] = torch.from_numpy(c)
+    gpos = torch.from_numpy(np.stack(gpos, 0)).to(dev)
+    return {
+        "bev_fts": bev_fts,
+        "bev_pos_fts": torch.cat([gpos.expand(-1, D * D, -1), trainer.bev_pos.expand(B, -1, -1, -1).reshape(B, -1, 3)],
+                                 -1),
         "bev_masks": torch.ones(B, D * D, dtype=torch.bool, device=dev),
         "bev_nav_masks": torch.from_numpy(nav_masks).to(dev),
         "bev_cand_idxs": bev_cand_idxs,

@@ -22,6 +22,14 @@ CE_SMALL = dict(num_l_layers=2, num_x_layers=2, num_pano_layers=1, vocab_size=30
                 attention_probs_dropout_prob=0.0, feat_dropout=0.0)
 
 
+# VLN-CE navigation (bevbert_ce/vlnce_baselines/models/bev/vlnbert_init.py:35-59 over bert-base-uncased): the keys
+# get_vlnbert_models sets, with depth embedding and graph sprels on (the R2R-CE run configs)
+CE_NAV_DEFAULTS = dict(R2R_DEFAULTS, image_feat_size=512, use_depth_embedding=True, depth_feat_size=128,
+                       angle_feat_size=4, graph_sprels=True, glocal_fuse="dynamic", fix_lang_embedding=False,
+                       fix_pano_embedding=False, output_attentions=True, pred_head_dropout_prob=0.1,
+                       use_lang2visn_attn=False, bev_dim=11, bev_res=1.0)
+
+
 def make_config(**overrides):
     """Returns a transformers.PretrainedConfig when transformers is importable (what the reference's
     BertPreTrainedModel subclasses need), else a SimpleNamespace with the same attributes."""
@@ -40,6 +48,16 @@ def make_config(**overrides):
 def make_ce_config(small=False, **overrides):
     """make_config for the VLN-CE model (model/ce_pretrain.py); `small` applies CE_SMALL before `overrides`."""
     vals = dict(CE_DEFAULTS)
+    if small:
+        vals.update(CE_SMALL)
+    vals.update(overrides)
+    return make_config(**vals)
+
+
+def make_ce_nav_config(small=False, **overrides):
+    """make_config for the VLN-CE navigation network (model/ce_nav.py); `small` applies CE_SMALL before `overrides`.
+    The reference's `use_sprels` is `graph_sprels` here, as in vlnbert_init.py."""
+    vals = dict(CE_NAV_DEFAULTS)
     if small:
         vals.update(CE_SMALL)
     vals.update(overrides)

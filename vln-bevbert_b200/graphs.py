@@ -19,7 +19,8 @@ A graph is keyed by (task, identity and shapes of the batch tensors).  sem / mas
 device-computed length, run in the model's `sync_free_mean` mode (mean over a device-side weight, same value and
 gradients); a step whose capture fails (a host synchronisation somewhere in forward) falls back to eager launches.
 
-`GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets.
+`GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets, and
+`install_ce_replay` the VLN-CE policy's.
 """
 import torch
 
@@ -212,27 +213,35 @@ def _round8(n):
     return (n + 7) // 8 * 8
 
 
-def nav_bucket(mode, batch):
-    """Graph key of a per-step call: mode, deterministic flag, and the padded shape and dtype of every input (B, object
-    presence, instruction length, map nodes, BEV candidates, object and panorama tokens)."""
+def _bucket(dims, mode, batch):
     key = [mode, torch.are_deterministic_algorithms_enabled()]
-    for name, dims in NAV_PAD_DIMS[mode].items():
+    for name, d in dims[mode].items():
         x = batch.get(name)
         if x is None:
             key.append(None)
         else:
-            key.append((tuple(_round8(n) if d in dims else n for d, n in enumerate(x.shape)), x.dtype))
+            key.append((tuple(_round8(n) if i in d else n for i, n in enumerate(x.shape)), x.dtype))
     return tuple(key)
 
 
-def nav_pad(mode, batch, device):
-    """The padded inputs a replay of `batch` computes on, as new zero-padded device tensors."""
+def _pad(dims, mode, batch, device):
     out = {}
-    for name, k in zip(NAV_PAD_DIMS[mode], nav_bucket(mode, batch)[2:]):
+    for name, k in zip(dims[mode], _bucket(dims, mode, batch)[2:]):
         if k is not None:
             out[name] = torch.zeros(k[0], dtype=k[1], device=device)
             out[name][tuple(slice(0, n) for n in batch[name].shape)] = batch[name]
     return out
+
+
+def nav_bucket(mode, batch):
+    """Graph key of a per-step call: mode, deterministic flag, and the padded shape and dtype of every input (B, object
+    presence, instruction length, map nodes, BEV candidates, object and panorama tokens)."""
+    return _bucket(NAV_PAD_DIMS, mode, batch)
+
+
+def nav_pad(mode, batch, device):
+    """The padded inputs a replay of `batch` computes on, as new zero-padded device tensors."""
+    return _pad(NAV_PAD_DIMS, mode, batch, device)
 
 
 def nav_slice(mode, out, batch):
@@ -268,6 +277,91 @@ def nav_forward_padded(model, mode, pad, host=None):
         p["bev_nav_masks"], p["bev_cand_idxs"], host[1], p.get("obj_embeds"), p.get("obj_masks"))
 
 
+class Surface:
+    """What GraphedNavigation needs to know about one per-step API: the padded dimensions of each call's inputs
+    (`dims`), the model on padded inputs (`padded(model, mode, pad, host)`), the outputs cut back to the caller's
+    shapes (`slice(mode, out, batch)`) and the unwrapped call (`eager(model, mode, batch)`)."""
+
+    def __init__(self, dims, padded, slice, eager):
+        self.dims, self.padded, self.slice, self.eager = dims, padded, slice, eager
+
+
+NAV = Surface(NAV_PAD_DIMS, nav_forward_padded, nav_slice,
+              lambda model, mode, batch: type(model).forward(model, mode, batch))
+
+
+# ------------------------------------------------------------------------------------ VLN-CE policy (model/ce_nav.py)
+# The CE policy calls three methods of its network; each is one mode here, its arguments the batch's keys.
+CE_NAV_CALLS = {
+    "forward_txt": ("language", ("txt_ids", "txt_masks")),
+    "forward_panorama": ("panorama", ("rgb_fts", "dep_fts", "loc_fts", "nav_types", "view_lens")),
+    "forward_navigation": ("navigation", ("txt_embeds", "txt_masks", "gmap_vpids", "gmap_step_ids", "gmap_img_fts",
+                                          "gmap_pos_fts", "gmap_masks", "gmap_visited_masks", "gmap_pair_dists",
+                                          "bev_fts", "bev_pos_fts", "bev_masks", "bev_nav_masks", "bev_cand_idxs",
+                                          "bev_cand_vpids")),
+}
+_CE_METHOD = {mode: name for name, (mode, _) in CE_NAV_CALLS.items()}
+CE_NAV_PAD_DIMS = {
+    "language": {"txt_ids": (1,), "txt_masks": (1,)},
+    "panorama": {"rgb_fts": (1,), "dep_fts": (1,), "loc_fts": (1,), "nav_types": (1,), "view_lens": ()},
+    "navigation": {"txt_embeds": (1,), "txt_masks": (1,), "gmap_step_ids": (1,), "gmap_img_fts": (1,),
+                   "gmap_pos_fts": (1,), "gmap_masks": (1,), "gmap_visited_masks": (1,), "gmap_pair_dists": (1, 2),
+                   "bev_fts": (), "bev_pos_fts": (), "bev_masks": (), "bev_nav_masks": (), "bev_cand_idxs": (1,)},
+}
+
+
+def ce_nav_bucket(mode, batch):
+    """nav_bucket of the CE calls: B exact (the CE rollout drops finished episodes), every other length rounded to 8"""
+    return _bucket(CE_NAV_PAD_DIMS, mode, batch)
+
+
+def ce_nav_pad(mode, batch, device):
+    return _pad(CE_NAV_PAD_DIMS, mode, batch, device)
+
+
+def ce_nav_eager(model, mode, batch):
+    """the network's own method (not an instance attribute that routes to a replay)"""
+    name = _CE_METHOD[mode]
+    return getattr(type(model), name)(model, *[batch[k] for k in CE_NAV_CALLS[name][1]])
+
+
+def ce_nav_forward_padded(model, mode, pad, host=None):
+    """the CE network on padded inputs `pad` (ce_nav_pad); `host` as for nav_forward_padded"""
+    if mode == "panorama":
+        return type(model).forward_panorama(model, *[pad.get(k) for k in CE_NAV_CALLS["forward_panorama"][1]],
+                                            vtot=pad["loc_fts"].shape[1])
+    if mode == "navigation":
+        pad = dict(pad, gmap_vpids=host[0], bev_cand_vpids=host[1])
+    return ce_nav_eager(model, mode, pad)
+
+
+def ce_nav_slice(mode, out, batch):
+    if mode != "navigation":
+        return nav_slice(mode, out, batch)
+    c = torch.Tensor.clone
+    G, Kc = batch["gmap_masks"].shape[1], batch["bev_cand_idxs"].shape[1]
+    return {"gmap_embeds": c(out["gmap_embeds"][:, :G]), "global_logits": c(out["global_logits"][:, :G]),
+            "local_logits": c(out["local_logits"][:, :Kc]), "fused_logits": c(out["fused_logits"][:, :G])}
+
+
+CE_NAV = Surface(CE_NAV_PAD_DIMS, ce_nav_forward_padded, ce_nav_slice, ce_nav_eager)
+
+
+def install_ce_replay(net):
+    """Routes the CE network's `forward_txt` / `forward_panorama` / `forward_navigation` through a GraphedNavigation
+    over the CE surface: eval-mode calls under torch.no_grad() replay graphs of padded shape buckets, every other call
+    runs the network's own method.  The module, its state_dict and its train / eval switch are unchanged.  Install on
+    the policy's network (`policy.net.vln_bert`); -> the GraphedNavigation (its `launches`, `entries`)."""
+    replay = GraphedNavigation(net, CE_NAV)
+    for name, (mode, args) in CE_NAV_CALLS.items():
+        def call(*a, _mode=mode, _args=args, **kw):
+            batch = dict(zip(_args, a))
+            batch.update(kw)
+            return replay(_mode, batch)
+        setattr(net, name, call)
+    return replay
+
+
 class GraphedNavigation:
     """The agents' per-step calls `model(mode, batch)` (GlocalTextPathNavCMT: language / panorama / navigation) replayed
     as CUDA graphs.  Called like the model, with the same inputs and outputs.
@@ -288,17 +382,18 @@ class GraphedNavigation:
     K-bucket).
 
     Agent side: `vln_bert.vln_bert.forward = GraphedNavigation(vln_bert.vln_bert)` keeps the module, its state_dict and
-    its train / eval switch, and routes its calls here."""
+    its train / eval switch, and routes its calls here.  `surface` names the per-step API (NAV, the agents'
+    `forward(mode, batch)`; CE_NAV, the CE policy's three methods, installed by `install_ce_replay`)."""
 
-    def __init__(self, model):
-        self.model = model
+    def __init__(self, model, surface=NAV):
+        self.model, self.s = model, surface
         self.params = list(model.parameters())
         self.entries = {}
         self.pool = None
         self.fresh = False
 
     def _eager(self, mode, batch):
-        return type(self.model).forward(self.model, mode, batch)
+        return self.s.eager(self.model, mode, batch)
 
     def _param_ptrs(self):
         return tuple(p.data_ptr() for p in self.params)
@@ -314,11 +409,11 @@ class GraphedNavigation:
         self.fresh = True
 
     def __call__(self, mode, batch):
-        if self.model.training or torch.is_grad_enabled() or mode not in NAV_PAD_DIMS:
+        if self.model.training or torch.is_grad_enabled() or mode not in self.s.dims:
             return self._eager(mode, batch)
         if mode == "language" or not self.fresh:
             self.refresh()
-        key = nav_bucket(mode, batch)
+        key = _bucket(self.s.dims, mode, batch)
         ent = self.entries.get(key)
         if ent is None:
             ent = self.entries[key] = self._new_entry(mode, batch)
@@ -338,12 +433,12 @@ class GraphedNavigation:
         ent["graph"].replay()
         if ent["stage"] is not None:
             ent["done"].record()
-        return nav_slice(mode, ent["out"], batch)
+        return self.s.slice(mode, ent["out"], batch)
 
     def _new_entry(self, mode, batch):
         dev = self.params[0].device
         bufs = {}
-        for name, k in zip(NAV_PAD_DIMS[mode], nav_bucket(mode, batch)[2:]):
+        for name, k in zip(self.s.dims[mode], _bucket(self.s.dims, mode, batch)[2:]):
             if k is not None:
                 bufs[name] = torch.zeros(k[0], dtype=k[1], device=dev)
         ent = {"in": bufs, "ext": {}, "graph": None, "out": None, "failed": False, "ptrs": None, "launches": None,
@@ -377,18 +472,18 @@ class GraphedNavigation:
     def _capture(self, ent, mode):
         torch.cuda.synchronize()
         # eager warm-up on the static buffers: weight shadows, packed biases, library workspaces, cuBLAS state
-        nav_forward_padded(self.model, mode, ent["in"], ent["host"])
+        self.s.padded(self.model, mode, ent["in"], ent["host"])
         torch.cuda.synchronize()
         if self.pool is None:
             self.pool = torch.cuda.graph_pool_handle()
         g = torch.cuda.CUDAGraph()
         n0 = K.launch_count()
         with torch.cuda.graph(g, pool=self.pool):
-            out = nav_forward_padded(self.model, mode, ent["in"], ent["host"])
+            out = self.s.padded(self.model, mode, ent["in"], ent["host"])
         ent["launches"] = K.launch_count() - n0
         ent["graph"], ent["out"], ent["ptrs"] = g, out, self._param_ptrs()
 
     def launches(self, mode, batch):
         """kernels of libbevbert_b200.so inside the graph of this call's bucket, or None when it runs eagerly."""
-        ent = self.entries.get(nav_bucket(mode, batch))
+        ent = self.entries.get(_bucket(self.s.dims, mode, batch))
         return ent["launches"] if ent is not None and ent["graph"] is not None else None
