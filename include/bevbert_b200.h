@@ -74,7 +74,7 @@ typedef struct bb_gemm_args {
   int32_t split_k;         /* >=1; >1 splits K across CTAs (D must be zeroed / hold the addend) */
   float alpha;
   const float* bias; /* [N] or NULL; added before the activation */
-  int32_t act;       /* 0 none, 1 exact-erf GELU, 2 ReLU */
+  int32_t act;       /* 0 none, 1 exact-erf GELU, 2 ReLU, 3 QuickGELU x*sigmoid(1.702x) (CLIP); others rejected */
   void* aux_out;     /* bf16, same strides as D: pre-activation (alpha*acc+bias) or NULL */
   const void* aux_in; /* bf16, same strides as D, or NULL */
   int32_t epi_mul;   /* 0 none; 1: result *= gelu'(aux_in); 2: result *= (aux_in > 0) */
@@ -252,6 +252,21 @@ int bb_add_rows(const void* a, const void* b, const float* table, const int64_t*
  * and reduces the table / vec gradients with bb_scatter_add_rows (or bb_scatter_rows_sorted) and bb_colsum_bf16. */
 int bb_add_rows3(const void* a, int64_t lda, const void* b, int64_t ldb, const void* c, int64_t ldc, const float* table,
                  const int64_t* idx, const float* vec, int64_t rows, int H, void* out, int64_t ldo, void* stream);
+/* ViT image tower input (csrc/vit.cu; OpenAI CLIP VisionTransformer, clip/model.py:206-237).
+ * bb_image_patches: the patch rows of the stride-P conv1 from N images of H x W x 3, pixel (n, y, x, c) at element
+ * n*sn + y*sh + x*sw + c*sc (NHWC as habitat delivers observations["rgb"]; an NCHW tensor is a permuted view), uint8
+ * (img_u8 = 1) or f32.  out ("bf16" activation, (N*(H/P)*(W/P), 3*P*P)): row (n*(H/P) + py)*(W/P) + px, column
+ * c*P*P + ky*P + kx (the flatten order of the (width, 3, P, P) weight).  Fused preprocessing, torchvision's
+ * ConvertImageDtype(float) + Normalize(mean, std) as torch computes them in fp32 on the device: a uint8 pixel times the
+ * fp32 reciprocal of 255, then (v - mean[c]) / std[c]; float pixels are not scaled.  mean / std: 3 host floats.
+ * H, W multiples of P; 3*P*P a multiple of 8; strides >= 0; out 16-byte and a float image 4-byte aligned.
+ * bb_vit_tokens: the first block's input, out ("bf16", (N*T, H)): row (n, 0) = LN(cls + pos[0]), row (n, t) =
+ * LN(patch[n*(T-1) + t-1] + pos[t]) (patch: f32 (N*(T-1), H), the conv GEMM's output; pos f32 (T, H)); LayerNorm in
+ * fp32 with gamma / beta, eps (ln_pre).  H % 8 == 0, H <= 1024, T >= 2, every pointer 16-byte aligned. */
+int bb_image_patches(const void* img, int img_u8, int N, int H, int W, int64_t sn, int64_t sh, int64_t sw, int64_t sc,
+                     int P, const float* mean, const float* std_, void* out, void* stream);
+int bb_vit_tokens(const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta,
+                  float eps, int N, int T, int H, void* out, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

@@ -130,18 +130,36 @@ class WeightCache:
             self._cast(ent)
         return ent.buf
 
+    def f32(self, p):
+        """fp32 copy of a 1-D parameter held in another dtype (CLIP's fp16 biases, clip/model.py:372-393), kept fresh
+        like the bf16 shadows (in place, so a CUDA graph that reads it sees `refresh_all(padded=True)`); an fp32
+        parameter is returned as it is."""
+        if p.dtype == torch.float32:
+            return p.detach()
+        key = ("f32", p.data_ptr())
+        ent = self._c.get(key)
+        if ent is not None and self._fresh(ent):
+            return ent.buf
+        if ent is None:
+            ent = self._c[key] = _Shadow((p,), torch.empty(p.shape, dtype=torch.float32, device=p.device), False)
+        self._cast(ent)
+        return ent.buf
+
     def _cast(self, ent):
-        if ent.plain:
+        if ent.plain and ent.params[0].dtype == torch.float32:
             r = 0
             for p in ent.params:
                 K.cast_to_act(p.detach(), out=ent.buf[r:r + p.shape[0]])
                 r += p.shape[0]
-        else:  # tiny padded operands: plain copies
-            k = ent.params[0].shape[1]
+        else:  # tiny padded operands, other source dtypes (fp16) and fp32 copies: plain copies, done once per change
             r = 0
-            for p in ent.params:
-                ent.buf[r:r + p.shape[0], :k] = p.detach().to(K.act_dtype())
-                r += p.shape[0]
+            with torch.no_grad():
+                for p in ent.params:
+                    dst = ent.buf[r:r + p.shape[0]]
+                    if p.dim() == 2:
+                        dst = dst[:, :p.shape[1]]
+                    dst.copy_(p.detach())
+                    r += p.shape[0]
         ent.ver, ent.epoch = tuple(p._version for p in ent.params), self.epoch
 
     def vec(self, *params):
@@ -182,9 +200,10 @@ class WeightCache:
         self.epoch += 1
         if padded:
             for e in self._c.values():
-                if not e.vec and (not e.plain or e.buf.dtype != torch.bfloat16):
+                if not e.vec and (not e.plain or e.buf.dtype != torch.bfloat16 or e.params[0].dtype != torch.float32):
                     self._cast(e)
-        ents = [e for e in self._c.values() if e.plain and not e.vec and e.buf.dtype == torch.bfloat16]
+        ents = [e for e in self._c.values() if e.plain and not e.vec and e.buf.dtype == torch.bfloat16
+                and e.params[0].dtype == torch.float32]
         if not ents or not ents[0].buf.is_cuda:
             return
         if self._table is None:
@@ -684,11 +703,13 @@ class XAttnImpl:
 
 class PanoLayerImpl:
     """Pre-norm TransformerEncoderLayer (transformer.py:170-182) with nn.MultiheadAttention's packed in_proj.
-    inputs (x (N,V,Hd), kmask (N,V) f32 with -inf on padding); params (in_w,in_b,out_w,out_b,l1w,l1b,l2w,l2b,
-    n1w,n1b,n2w,n2b)."""
+    inputs (x (N,V,Hd), kmask (N,V) f32 with -inf on padding, or None); params (in_w,in_b,out_w,out_b,l1w,l1b,l2w,l2b,
+    n1w,n1b,n2w,n2b).  `act` is the FFN activation: K.ACT_GELU (the panorama encoder), or K.ACT_QGELU for CLIP's
+    ResidualAttentionBlock (clip/model.py:167-188), which runs forward only: the composed launches without the
+    pre-activation copy, and no backward."""
 
-    def __init__(self, rt, heads, p_attn=0.0, p_hidden=0.0):
-        self.rt, self.wc, self.H, self.pa, self.ph = rt, rt.wc, heads, p_attn, p_hidden
+    def __init__(self, rt, heads, p_attn=0.0, p_hidden=0.0, act=K.ACT_GELU):
+        self.rt, self.wc, self.H, self.pa, self.ph, self.act = rt, rt.wc, heads, p_attn, p_hidden, act
 
     def _native_fwd(self, st, x, kmask, p):
         wc, ds = self.wc, self.rt.ds
@@ -736,7 +757,7 @@ class PanoLayerImpl:
 
     def fwd(self, st, inputs, p):
         x, kmask = inputs
-        st["native"] = K.native_sublayers()
+        st["native"] = self.act == K.ACT_GELU and K.native_sublayers()
         if st["native"]:
             return self._native_fwd(st, x, kmask, p)
         N, V, Hd = x.shape
@@ -751,7 +772,8 @@ class PanoLayerImpl:
         x1, _ = lin_fwd(ctx, self.wc.get(p[2]), p[3].detach(), drop=d1, add_in=x2)
         h2, _, m2, r2 = K.layernorm_fwd(x1, None, p[10].detach(), p[11].detach(), 1e-5)
         d2 = self.rt.ds.make(self.ph)
-        f, fpre = lin_fwd(h2, self.wc.get(p[4]), p[5].detach(), act=K.ACT_GELU, want_pre=True, drop=d2)
+        gelu = self.act == K.ACT_GELU
+        f, fpre = lin_fwd(h2, self.wc.get(p[4]), p[5].detach(), act=self.act, want_pre=gelu, drop=d2)
         d3 = self.rt.ds.make(self.ph)
         y, _ = lin_fwd(f, self.wc.get(p[6]), p[7].detach(), drop=d3, add_in=x1)
         st.update(x2=x2, h1=h1, m1=m1, r1=r1, qkv=qkv, ctx=ctx, x1=x1, h2=h2, m2=m2, r2=r2, f=f, fpre=fpre, d1=d1,
@@ -761,6 +783,8 @@ class PanoLayerImpl:
     def bwd(self, st, gouts, p):
         if st["native"]:
             return self._native_bwd(st, gouts[0])
+        if self.act != K.ACT_GELU:
+            raise NotImplementedError("PanoLayerImpl runs backward with GELU only")
         Hd = st["shape"][-1]
         dev = st["x2"].device
         dy = gouts[0].reshape(-1, Hd).contiguous()

@@ -90,6 +90,7 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const F32Params p) {
       if (p.aux_out) p.aux_out[off] = v;
       if (p.act == 1) v = gelu_erf(v);
       else if (p.act == 2) v = fmaxf(v, 0.f);
+      else if (p.act == 3) v = qgelu(v);
       if (p.epi_mul == 1) v *= dgelu_erf(p.aux_in[off]);
       else if (p.epi_mul == 2) v = p.aux_in[off] > 0.f ? v : 0.f;
       if (p.drop_thresh) v = drop_keep(p.drop_seed, (uint64_t)off, p.drop_thresh) ? v * p.drop_scale : 0.f;

@@ -233,6 +233,7 @@ __device__ __forceinline__ void epi_chunk(const GemmKParams& p, long long off, i
   for (int i = 0; i < 8; ++i) {
     if (act == 1) v[i] = fast_gelu ? gelu_fast(v[i]) : gelu_erf(v[i]);
     else if (act == 2) v[i] = fmaxf(v[i], 0.0f);
+    else if (act == 3) v[i] = qgelu(v[i]);
     if (mul == 1) v[i] *= fast_gelu ? dgelu_fast(bf16_at(mul_in, i)) : dgelu_erf(bf16_at(mul_in, i));
     else if (mul == 2) v[i] = bf16_at(mul_in, i) > 0.0f ? v[i] : 0.0f;
     if (drop) v[i] = drop_keep(p.drop_seed, (uint64_t)(off + i), p.drop_thresh) ? v[i] * p.drop_scale : 0.0f;
@@ -737,6 +738,7 @@ int gemm_f32_launch(const bb_gemm_args* a, cudaStream_t stream);   // fp32 verif
 extern "C" int bb_gemm_bf16(const bb_gemm_args* a, void* stream_) {
   using namespace bb;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (a && (a->act < 0 || a->act > 3)) return set_error("bb_gemm_bf16: act must be 0 (none), 1 (GELU), 2 (ReLU) or 3 (QuickGELU)");
   if (act_f32()) return gemm_f32_launch(a, stream);
   if (!a || !a->A || !a->B || !a->D) return set_error("bb_gemm_bf16: null argument");
   if (a->M <= 0 || a->N <= 0 || a->K <= 0) return set_error("bb_gemm_bf16: M, N, K must be positive");

@@ -168,6 +168,10 @@ __device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (
 
 // ---------------------------------------------------------------- misc math
 __device__ __forceinline__ float gelu_erf(float x) { return x * 0.5f * (1.0f + erff(x * 0.70710678118654752440f)); }
+// QuickGELU of OpenAI CLIP, x * sigmoid(1.702 x) (clip/model.py QuickGELU): x / (1 + e^(-1.702 x)) with the full-range
+// expf and a correctly rounded division, so the result stays within a few fp32 ulps of the exact value for every x
+// (for x below about -52 the exponential overflows and the result is -0).
+__device__ __forceinline__ float qgelu(float x) { return __fdiv_rn(x, 1.0f + expf(-1.702f * x)); }
 __device__ __forceinline__ float dgelu_erf(float x) {
   const float cdf = 0.5f * (1.0f + erff(x * 0.70710678118654752440f));
   const float pdf = 0.39894228040143267794f * __expf(-0.5f * x * x);

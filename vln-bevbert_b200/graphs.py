@@ -19,8 +19,8 @@ A graph is keyed by (task, identity and shapes of the batch tensors).  sem / mas
 device-computed length, run in the model's `sync_free_mean` mode (mean over a device-side weight, same value and
 gradients); a step whose capture fails (a host synchronisation somewhere in forward) falls back to eager launches.
 
-`GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets, and
-`install_ce_replay` the VLN-CE policy's.
+`GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets,
+`install_ce_replay` the VLN-CE policy's, and `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder.
 """
 import torch
 
@@ -280,10 +280,13 @@ def nav_forward_padded(model, mode, pad, host=None):
 class Surface:
     """What GraphedNavigation needs to know about one per-step API: the padded dimensions of each call's inputs
     (`dims`), the model on padded inputs (`padded(model, mode, pad, host)`), the outputs cut back to the caller's
-    shapes (`slice(mode, out, batch)`) and the unwrapped call (`eager(model, mode, batch)`)."""
+    shapes (`slice(mode, out, batch)`) and the unwrapped call (`eager(model, mode, batch)`).  `grad_ok`: eval-mode
+    calls replay with grad enabled too (a frozen, forward-only model); `stale(model)`: True when the weights changed
+    since the previous call, so that every call, not only `language`, re-casts the shadows first."""
 
-    def __init__(self, dims, padded, slice, eager):
+    def __init__(self, dims, padded, slice, eager, grad_ok=False, stale=None):
         self.dims, self.padded, self.slice, self.eager = dims, padded, slice, eager
+        self.grad_ok, self.stale = grad_ok, stale
 
 
 NAV = Surface(NAV_PAD_DIMS, nav_forward_padded, nav_slice,
@@ -362,6 +365,36 @@ def install_ce_replay(net):
     return replay
 
 
+# ------------------------------------------------------------------- VLN-CE policy RGB encoder (model/clip_visual.py)
+# One mode; the input is observations["rgb"] at its exact shape (N = 12 views x B environments) and dtype.
+CE_RGB_DIMS = {"rgb": {"rgb": ()}}
+CE_RGB = Surface(CE_RGB_DIMS, lambda tower, mode, pad, host=None: tower.encode_rgb(pad["rgb"]),
+                 lambda mode, out, batch: (out[0].clone(), out[1].clone()),
+                 lambda tower, mode, batch: tower.encode_rgb(batch["rgb"]),
+                 grad_ok=True, stale=lambda tower: tower.changed())
+
+
+def install_ce_rgb_encoder(rgb_encoder):
+    """Routes the CE policy's `CLIPEncoderB16` instance (`policy.net.rgb_encoder`, `policy.net.module.rgb_encoder`
+    with data parallelism) to the kernels: `rgb_encoder(observations)` returns (rgb_vector, rgb_grid) as fresh fp32
+    tensors, computed by model.clip_visual.ClipTower from the weights of `rgb_encoder.model.visual` with the mean / std
+    of its `rgb_transform`.  While the encoder is in eval mode every call, with or without grad, replays the CUDA graph
+    of its image count N (one graph per N; N = 12 B shrinks as episodes finish) on a static copy of
+    observations["rgb"]; in training mode, or if a capture fails, the same kernels run eagerly.  A weight change
+    (load_state_dict) is seen by the next call either way.  The module, the policy's state_dict, checkpoints and the
+    train / eval switch are unchanged.  -> the GraphedNavigation (its `launches`, `entries`)."""
+    from .model.clip_visual import ClipTower
+    norm = rgb_encoder.rgb_transform[-1]
+    tower = ClipTower(rgb_encoder.model.visual, mean=norm.mean, std=norm.std, owner=rgb_encoder)
+    replay = GraphedNavigation(tower, CE_RGB)
+
+    def forward(observations):
+        tower.check_grad()
+        return replay("rgb", {"rgb": observations["rgb"]})
+    rgb_encoder.forward = forward
+    return replay
+
+
 class GraphedNavigation:
     """The agents' per-step calls `model(mode, batch)` (GlocalTextPathNavCMT: language / panorama / navigation) replayed
     as CUDA graphs.  Called like the model, with the same inputs and outputs.
@@ -409,9 +442,9 @@ class GraphedNavigation:
         self.fresh = True
 
     def __call__(self, mode, batch):
-        if self.model.training or torch.is_grad_enabled() or mode not in self.s.dims:
+        if self.model.training or (torch.is_grad_enabled() and not self.s.grad_ok) or mode not in self.s.dims:
             return self._eager(mode, batch)
-        if mode == "language" or not self.fresh:
+        if mode == "language" or not self.fresh or (self.s.stale is not None and self.s.stale(self.model)):
             self.refresh()
         key = _bucket(self.s.dims, mode, batch)
         ent = self.entries.get(key)

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib
 
-ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
+ACT_NONE, ACT_GELU, ACT_RELU, ACT_QGELU = 0, 1, 2, 3     # ACT_QGELU: x * sigmoid(1.702 x), CLIP
 EPI_NONE, EPI_DGELU, EPI_DRELU = 0, 1, 2
 BF16 = torch.bfloat16
 

@@ -402,3 +402,43 @@ def split_batch(batch: dict, parts: int):
                 sub[k] = v[lo:hi]
         out.append(sub)
     return out
+
+
+CLIP_B16 = dict(input_resolution=224, patch_size=16, width=768, layers=12, heads=12, output_dim=512)
+_CLIP_FP16 = ("conv1.weight", "proj", "in_proj_weight", "in_proj_bias", "out_proj.weight", "out_proj.bias",
+              "c_fc.weight", "c_fc.bias", "c_proj.weight", "c_proj.bias")
+
+
+def clip_visual_state(seed: int = 0, input_resolution=224, patch_size=16, width=768, layers=12, heads=12,
+                      output_dim=512):
+    """Seeded state_dict of CLIP's ViT image tower (clip/model.py VisionTransformer keys, in its state_dict order),
+    machine-independent (det_uniform).  Scales follow CLIP's own: embeddings and proj width^-0.5 (VisionTransformer's
+    constructor); in_proj / out_proj / c_fc / c_proj with initialize_parameters' attn_std, proj_std and fc_std; conv1
+    (3 P^2)^-0.5.  Biases are small but non-zero and LayerNorms are perturbed around (1, 0), so that every term of the
+    forward is exercised.  Tensors are fp32, rounded to fp16 where clip's convert_weights stores fp16."""
+    D, P, L = width, patch_size, layers
+    attn_std, proj_std, fc_std = D ** -0.5, D ** -0.5 * (2 * L) ** -0.5, (2 * D) ** -0.5
+    shapes = [("class_embedding", (D,), D ** -0.5), ("positional_embedding", ((input_resolution // P) ** 2 + 1, D),
+                                                      D ** -0.5),
+              ("proj", (D, output_dim), D ** -0.5), ("conv1.weight", (D, 3, P, P), (3 * P * P) ** -0.5),
+              ("ln_pre.weight", (D,), "ln"), ("ln_pre.bias", (D,), 0.05)]
+    for i in range(L):
+        b = "transformer.resblocks.%d." % i
+        shapes += [(b + "attn.in_proj_weight", (3 * D, D), attn_std), (b + "attn.in_proj_bias", (3 * D,), 0.02),
+                   (b + "attn.out_proj.weight", (D, D), proj_std), (b + "attn.out_proj.bias", (D,), 0.02),
+                   (b + "ln_1.weight", (D,), "ln"), (b + "ln_1.bias", (D,), 0.05),
+                   (b + "mlp.c_fc.weight", (4 * D, D), fc_std), (b + "mlp.c_fc.bias", (4 * D,), 0.02),
+                   (b + "mlp.c_proj.weight", (D, 4 * D), proj_std), (b + "mlp.c_proj.bias", (D,), 0.02),
+                   (b + "ln_2.weight", (D,), "ln"), (b + "ln_2.bias", (D,), 0.05)]
+    shapes += [("ln_post.weight", (D,), "ln"), ("ln_post.bias", (D,), 0.05)]
+    sd = {}
+    for j, (k, shape, std) in enumerate(shapes):
+        a = (0.1 if std == "ln" else std) * math.sqrt(3.0)
+        v = det_uniform(shape, seed, 7000 + j, -a, a) + (1.0 if std == "ln" else 0.0)
+        sd[k] = v.half().float() if k.endswith(_CLIP_FP16) else v
+    return sd
+
+
+def clip_images(n: int, seed: int = 0, res: int = 224) -> torch.Tensor:
+    """n seeded uint8 RGB observations (n, res, res, 3), as habitat delivers observations["rgb"]"""
+    return det_randint((n, res, res, 3), seed, 7999, 0, 255).to(torch.uint8)
