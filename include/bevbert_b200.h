@@ -267,6 +267,15 @@ int bb_image_patches(const void* img, int img_u8, int N, int H, int W, int64_t s
                      int P, const float* mean, const float* std_, void* out, void* stream);
 int bb_vit_tokens(const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta,
                   float eps, int N, int T, int H, void* out, void* stream);
+/* Waypoint heatmap NMS (csrc/waypoint.cu; bevbert_ce/vlnce_baselines/waypoint_pred/utils.py nms with gaussian=False,
+ * called at models/Policy_ViewSelection_BEV.py:221).  pred, out: f32 (B, H, W) contiguous, not overlapping.  For each
+ * of max_predictions rounds and each row b: ix = argmax of the suppressed map (torch.max's rules: NaN is the maximum,
+ * the lowest index wins ties, -0.0 == +0.0); out[b, ix] = pred[b, ix]; then the suppressed map is multiplied by
+ * (1 - g) in fp32, g = 1 where |y - ix/W| <= sigma_y (true division) and min(|x - ix%W|, |x - ix%W + W|) <= sigma_x.
+ * Every other cell of out is 0 and negative outputs are clamped to +0.  Bit-identical to the reference on the CPU.
+ * B, H, W > 0; H * W <= 8192; max_predictions >= 0 (0: out is all zeros); pointers 4-byte aligned. */
+int bb_waypoint_nms(const float* pred, int B, int H, int W, float sigma_x, float sigma_y, int max_predictions,
+                    float* out, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

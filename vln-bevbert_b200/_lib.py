@@ -142,6 +142,7 @@ _SIGNATURES = {
     "bb_image_patches": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_i64, c_i64, c_i64, c_i64, c_int,
                                  C.POINTER(c_float), C.POINTER(c_float), c_void_p, c_void_p]),
     "bb_vit_tokens": (c_int, [c_void_p] * 5 + [c_float, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "bb_waypoint_nms": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_int, c_void_p, c_void_p]),
     "bb_scale_rows_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p]),
     "bb_segment_wsum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_segment_wsum_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),

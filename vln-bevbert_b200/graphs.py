@@ -20,7 +20,8 @@ device-computed length, run in the model's `sync_free_mean` mode (mean over a de
 gradients); a step whose capture fails (a host synchronisation somewhere in forward) falls back to eager launches.
 
 `GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets,
-`install_ce_replay` the VLN-CE policy's, and `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder.
+`install_ce_replay` the VLN-CE policy's, `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder, and
+`install_ce_waypoint_predictor` the CE trainer's waypoint predictor.
 """
 import torch
 
@@ -392,6 +393,39 @@ def install_ce_rgb_encoder(rgb_encoder):
         tower.check_grad()
         return replay("rgb", {"rgb": observations["rgb"]})
     rgb_encoder.forward = forward
+    return replay
+
+
+# ------------------------------------------------------------------------ VLN-CE waypoint predictor (model/waypoint.py)
+# One mode; the input is the depth features at their exact shape (N = 12 views x B environments) and dtype.  rgb_feats
+# only decides B, which the depth features' N repeats, so it is not copied into the graph's buffers.
+CE_WAYPOINT_DIMS = {"waypoint": {"depth_feats": ()}}
+CE_WAYPOINT = Surface(CE_WAYPOINT_DIMS, lambda runner, mode, pad, host=None: runner.logits(pad["depth_feats"]),
+                      lambda mode, out, batch: out.clone(),
+                      lambda runner, mode, batch: runner.logits(batch["depth_feats"]),
+                      grad_ok=True, stale=lambda runner: runner.changed())
+
+
+def install_ce_waypoint_predictor(waypoint_predictor):
+    """Routes the trainer's waypoint predictor (TRM_net.py BinaryDistPredictor_TRM; under nn.DataParallel the wrapped
+    `.module`) to the kernels: `waypoint_predictor(rgb_feats, depth_feats)` returns the heatmap logits (B, 120, 12) as
+    a fresh fp32 tensor, computed by model.waypoint.WaypointRunner from the module's own weights.  Every eval-mode call,
+    with or without grad (the trainer freezes the predictor), replays the CUDA graph of its view count N (one graph per
+    N = 12 B) on a static copy of depth_feats; a capture that fails runs the same kernels eagerly.  A call in training
+    mode, or with grad enabled while a parameter requires grad, raises.  A weight change (load_state_dict) is seen by
+    the next call.  The module, its state_dict and its train / eval switch are unchanged.  -> the GraphedNavigation
+    (its `launches`, `entries`)."""
+    from .model.waypoint import WaypointRunner
+    module = waypoint_predictor
+    if isinstance(module, (torch.nn.DataParallel, torch.nn.parallel.DistributedDataParallel)):
+        module = module.module
+    runner = WaypointRunner(module)
+    replay = GraphedNavigation(runner, CE_WAYPOINT)
+
+    def forward(rgb_feats, depth_feats):
+        runner.check_call()
+        return replay("waypoint", {"depth_feats": runner.check_inputs(rgb_feats, depth_feats)})
+    module.forward = forward
     return replay
 
 

@@ -442,3 +442,33 @@ def clip_visual_state(seed: int = 0, input_resolution=224, patch_size=16, width=
 def clip_images(n: int, seed: int = 0, res: int = 224) -> torch.Tensor:
     """n seeded uint8 RGB observations (n, res, res, 3), as habitat delivers observations["rgb"]"""
     return det_randint((n, res, res, 3), seed, 7999, 0, 255).to(torch.uint8)
+
+
+def waypoint_state(seed: int = 0):
+    """Seeded state_dict of the VLN-CE waypoint predictor (waypoint_pred/TRM_net.py BinaryDistPredictor_TRM keys, in its
+    state_dict order, the unused visual_merge / mergefeats_LayerNorm included), machine-independent (det_uniform).
+    Linear weights are uniform with standard deviation fan_in^-0.5, biases small but non-zero, LayerNorms perturbed
+    around (1, 0), so that logits stay O(1) and every term of the forward is exercised."""
+    D, F = 768, 3072
+    shapes = [("visual_fc_depth.1.weight", (D, 2048), 2048 ** -0.5), ("visual_fc_depth.1.bias", (D,), 0.02),
+              ("visual_merge.0.weight", (D, 2 * D), (2 * D) ** -0.5), ("visual_merge.0.bias", (D,), 0.02)]
+    for i in range(2):
+        b = "waypoint_TRM.bert.encoder.layer.%d." % i
+        for name in ("query", "key", "value"):
+            shapes += [(b + "attention.self.%s.weight" % name, (D, D), D ** -0.5),
+                       (b + "attention.self.%s.bias" % name, (D,), 0.02)]
+        shapes += [(b + "attention.output.dense.weight", (D, D), D ** -0.5),
+                   (b + "attention.output.dense.bias", (D,), 0.02),
+                   (b + "attention.output.LayerNorm.weight", (D,), "ln"),
+                   (b + "attention.output.LayerNorm.bias", (D,), 0.05),
+                   (b + "intermediate.dense.weight", (F, D), D ** -0.5), (b + "intermediate.dense.bias", (F,), 0.02),
+                   (b + "output.dense.weight", (D, F), F ** -0.5), (b + "output.dense.bias", (D,), 0.02),
+                   (b + "output.LayerNorm.weight", (D,), "ln"), (b + "output.LayerNorm.bias", (D,), 0.05)]
+    shapes += [("mergefeats_LayerNorm.weight", (D,), "ln"), ("mergefeats_LayerNorm.bias", (D,), 0.05),
+               ("vis_classifier.0.weight", (D, D), D ** -0.5), ("vis_classifier.0.bias", (D,), 0.02),
+               ("vis_classifier.2.weight", (120, D), D ** -0.5), ("vis_classifier.2.bias", (120,), 0.02)]
+    sd = {}
+    for j, (k, shape, std) in enumerate(shapes):
+        a = (0.1 if std == "ln" else std) * math.sqrt(3.0)
+        sd[k] = det_uniform(shape, seed, 8000 + j, -a, a) + (1.0 if std == "ln" else 0.0)
+    return sd
