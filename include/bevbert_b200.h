@@ -276,6 +276,30 @@ int bb_vit_tokens(const float* patch, const float* cls, const float* pos, const 
  * B, H, W > 0; H * W <= 8192; max_predictions >= 0 (0: out is all zeros); pointers 4-byte aligned. */
 int bb_waypoint_nms(const float* pred, int B, int H, int W, float sigma_x, float sigma_y, int max_predictions,
                     float* out, void* stream);
+/* Depth encoder of the VLN-CE policy (csrc/conv.cu; resnet_encoders.py:13-107 VlnResnetDepthEncoder over the DD-PPO
+ * GroupNorm ResNet-50).  Activations are NHWC, fp16 in the product path and fp32 in the verification arm
+ * (bb_set_act_f32).  GroupNorm partials: a map of rows m = (n, h, w) with C channels and G groups gets, per stat tile
+ * of tm consecutive rows, per image j the tile touches (j counted from the tile's first image) and per channel block of
+ * cb = min(C / G, 32) channels, one f32 {count, mean, M2, 0} of the stored values, at float4 index
+ * (tile * SEG + j) * (C / cb) + block, SEG = (tm + H*W - 2) / (H*W) + 1; no atomics.
+ * bb_conv2d: y (N, Ho, Wo, Cout) = conv(x (N, H, W, Cin), w (Cout, R, R, Cin)), no bias, R = 1 or 3, stride 1 or 2, pad
+ * (R - 1) / 2; fp16 operands on wgmma with fp32 accumulation (a CUDA-core fp32 convolution in the arm); partials with
+ * tm = 128.  Cin % 16 == 0, Cout % 32 == 0, groups divides Cout, C / G divides 32 or is a multiple of 32, 16-byte alignment.
+ * bb_depth_stem: avg_pool2d(depth, 2) of the f32 depth (N, Hd, Wd), element (n, h, w) at n*sn + h*sh + w*sw, then the
+ * 7x7 / 2, pad 3 convolution with w f32 (32, 1, 7, 7) -> y (N, Ho, Wo, 32); partials with tm = Wo; Wo <= 256.
+ * bb_groupnorm_apply: out = relu(gamma (x - mean) rstd + beta) with mode 0; + identity before the relu with mode 1;
+ * + gamma2 (x2 - mean2) rstd2 + beta2 (x2's own partials, tile height tm2) with mode 2; mode 3 max-pools the mode-0
+ * result 3x3 / 2, pad 1, into (N, (H-1)/2+1, (W-1)/2+1, C).  Mean and variance per (image, group) combine the partials
+ * in a fixed order with Chan's rule; eps as GroupNorm.  out_f32 = 1 (mode 0 only) writes f32 (N, C, H, W), the encoder's
+ * output dtype and layout, in either path.
+ * C % 8 == 0, C <= 1024, groups <= 32, 16-byte alignment. */
+int bb_conv2d(const void* x, const void* w, int N, int H, int W, int Cin, int Cout, int R, int stride, int groups,
+              void* y, void* stats, void* stream);
+int bb_depth_stem(const float* depth, int N, int Hd, int Wd, int64_t sn, int64_t sh, int64_t sw, const float* w,
+                  int groups, void* y, void* stats, void* stream);
+int bb_groupnorm_apply(const void* x, const void* stats, int tm, const float* gamma, const float* beta, const void* x2,
+                       const void* stats2, int tm2, const float* gamma2, const float* beta2, const void* identity, int N,
+                       int H, int W, int C, int groups, float eps, int mode, int out_f32, void* out, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

@@ -143,6 +143,11 @@ _SIGNATURES = {
                                  C.POINTER(c_float), C.POINTER(c_float), c_void_p, c_void_p]),
     "bb_vit_tokens": (c_int, [c_void_p] * 5 + [c_float, c_int, c_int, c_int, c_void_p, c_void_p]),
     "bb_waypoint_nms": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_int, c_void_p, c_void_p]),
+    "bb_conv2d": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p] * 3),
+    "bb_depth_stem": (c_int, [c_void_p, c_int, c_int, c_int, c_i64, c_i64, c_i64, c_void_p, c_int, c_void_p, c_void_p,
+                              c_void_p]),
+    "bb_groupnorm_apply": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                   c_void_p, c_void_p] + [c_int] * 5 + [c_float, c_int, c_int, c_void_p, c_void_p]),
     "bb_scale_rows_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p]),
     "bb_segment_wsum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_segment_wsum_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),

@@ -78,10 +78,11 @@ class Runtime:
 
 
 class _Shadow:
-    __slots__ = ("params", "buf", "ver", "epoch", "plain", "vec")
+    __slots__ = ("params", "buf", "ver", "epoch", "plain", "vec", "view")
 
-    def __init__(self, params, buf, plain, vec=False):
+    def __init__(self, params, buf, plain, vec=False, view=None):
         self.params, self.buf, self.plain, self.vec = params, buf, plain, vec
+        self.view = view            # copy source of a re-laid-out shadow: view(param) has buf's shape
         self.ver, self.epoch = None, -1
 
 
@@ -145,6 +146,20 @@ class WeightCache:
         self._cast(ent)
         return ent.buf
 
+    def conv_nhwc(self, p, dtype):
+        """A conv weight (Cout, Cin, R, S) as a (Cout, R, S, Cin) `dtype` copy (the depth encoder's fp16 implicit-GEMM
+        operand, fp32 in the verification arm), kept fresh like the other shadows (in place, so a CUDA graph that reads
+        it sees `refresh_all(padded=True)`)."""
+        key = ("nhwc", p.data_ptr(), dtype)
+        ent = self._c.get(key)
+        if ent is not None and self._fresh(ent):
+            return ent.buf
+        if ent is None:
+            buf = torch.empty(p.shape[0], p.shape[2], p.shape[3], p.shape[1], dtype=dtype, device=p.device)
+            ent = self._c[key] = _Shadow((p,), buf, False, view=lambda t: t.permute(0, 2, 3, 1))
+        self._cast(ent)
+        return ent.buf
+
     def _cast(self, ent):
         if ent.plain and ent.params[0].dtype == torch.float32:
             r = 0
@@ -158,7 +173,7 @@ class WeightCache:
                     dst = ent.buf[r:r + p.shape[0]]
                     if p.dim() == 2:
                         dst = dst[:, :p.shape[1]]
-                    dst.copy_(p.detach())
+                    dst.copy_(p.detach() if ent.view is None else ent.view(p.detach()))
                     r += p.shape[0]
         ent.ver, ent.epoch = tuple(p._version for p in ent.params), self.epoch
 

@@ -20,8 +20,9 @@ device-computed length, run in the model's `sync_free_mean` mode (mean over a de
 gradients); a step whose capture fails (a host synchronisation somewhere in forward) falls back to eager launches.
 
 `GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets,
-`install_ce_replay` the VLN-CE policy's, `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder, and
-`install_ce_waypoint_predictor` the CE trainer's waypoint predictor.
+`install_ce_replay` the VLN-CE policy's, `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder,
+`install_ce_depth_encoder` its ResNet-50 depth encoder, and `install_ce_waypoint_predictor` the CE trainer's waypoint
+predictor.
 """
 import torch
 
@@ -426,6 +427,38 @@ def install_ce_waypoint_predictor(waypoint_predictor):
         runner.check_call()
         return replay("waypoint", {"depth_feats": runner.check_inputs(rgb_feats, depth_feats)})
     module.forward = forward
+    return replay
+
+
+# ------------------------------------------------------------------ VLN-CE policy depth encoder (model/depth_resnet.py)
+# One mode; the input is observations["depth"] at its exact shape (N = 12 views x B environments) and dtype.
+CE_DEPTH_DIMS = {"depth": {"depth": ()}}
+CE_DEPTH = Surface(CE_DEPTH_DIMS, lambda tower, mode, pad, host=None: tower.encode(pad["depth"]),
+                   lambda mode, out, batch: out.clone(),
+                   lambda tower, mode, batch: tower.encode(batch["depth"]),
+                   grad_ok=True, stale=lambda tower: tower.changed())
+
+
+def install_ce_depth_encoder(depth_encoder):
+    """Routes the CE policy's `VlnResnetDepthEncoder` instance (`policy.net.depth_encoder`,
+    `policy.net.module.depth_encoder` with data parallelism) to the kernels: its `visual_encoder(observations)` returns
+    the (N, 128, 4, 4) features as a fresh fp32 tensor, computed by model.depth_resnet.DepthTower from the weights of
+    `depth_encoder.visual_encoder`, so the wrapper's own `depth_features` and `spatial_output` branches are unchanged.
+    While the encoder is in eval mode every call, with or without grad, replays the CUDA graph of its image count N (one
+    graph per N; N = 12 B shrinks as episodes finish) on a static copy of observations["depth"]; in training mode, or if
+    a capture fails, the same kernels run eagerly.  A call with grad enabled while an encoder parameter requires grad
+    (trainable=True) raises.  A weight change (load_state_dict) is seen by the next call either way.  The module, the
+    policy's state_dict, checkpoints and the train / eval switch are unchanged.  -> the GraphedNavigation (its
+    `launches`, `entries`)."""
+    from .model.depth_resnet import DepthTower
+    visual = depth_encoder.visual_encoder
+    tower = DepthTower(visual, owner=depth_encoder)
+    replay = GraphedNavigation(tower, CE_DEPTH)
+
+    def forward(observations):
+        tower.check_grad()
+        return replay("depth", {"depth": observations["depth"]})
+    visual.forward = forward
     return replay
 
 

@@ -472,3 +472,44 @@ def waypoint_state(seed: int = 0):
         a = (0.1 if std == "ln" else std) * math.sqrt(3.0)
         sd[k] = det_uniform(shape, seed, 8000 + j, -a, a) + (1.0 if std == "ln" else 0.0)
     return sd
+
+
+def depth_encoder_state(seed: int = 0, height=256, width=256):
+    """Seeded state_dict of the VLN-CE policy's depth encoder (model.depth_resnet.depth_encoder(): habitat-lab's
+    ResNetEncoder over resnet50 with 32 base planes and GroupNorm(16); keys in its state_dict order),
+    machine-independent (det_uniform).  Conv weights are uniform with He's standard deviation (2 / fan_in)^0.5;
+    GroupNorm weights are perturbed around 1 and biases around 0, so that every term of the forward is exercised."""
+    from .model.depth_resnet import depth_encoder
+    sd = {}
+    for j, (k, v) in enumerate(depth_encoder(height, width).state_dict().items()):
+        if v.dim() == 4:
+            a = (2.0 / (v[0].numel())) ** 0.5 * math.sqrt(3.0)
+            sd[k] = det_uniform(tuple(v.shape), seed, 9000 + j, -a, a)
+        elif k.endswith("weight"):
+            a = 0.1 * math.sqrt(3.0)
+            sd[k] = det_uniform(tuple(v.shape), seed, 9000 + j, 1.0 - a, 1.0 + a)
+        else:
+            a = 0.05 * math.sqrt(3.0)
+            sd[k] = det_uniform(tuple(v.shape), seed, 9000 + j, -a, a)
+    return sd
+
+
+def ddppo_checkpoint(seed: int = 0):
+    """A DD-PPO checkpoint as VlnResnetDepthEncoder loads it (resnet_encoders.py:38-47): {"state_dict": ...} with the
+    depth_encoder_state(seed) weights under `actor_critic.net.visual_encoder.*`, plus keys of the policy's other parts
+    that the loader must skip."""
+    sd = {"actor_critic.net.prev_action_embedding.weight": det_uniform((5, 32), seed, 9900, -1.0, 1.0)}
+    for k, v in depth_encoder_state(seed).items():
+        sd["actor_critic.net.visual_encoder." + k] = v
+    sd["actor_critic.net.visual_fc.1.weight"] = det_uniform((512, 2048), seed, 9901, -0.01, 0.01)
+    sd["actor_critic.net.state_encoder.rnn.weight_ih_l0"] = det_uniform((2048, 544), seed, 9902, -0.01, 0.01)
+    sd["actor_critic.net.state_encoder.rnn.bias_ih_l0"] = det_uniform((2048,), seed, 9903, -0.01, 0.01)
+    sd["actor_critic.action_distribution.linear.weight"] = det_uniform((4, 512), seed, 9904, -0.01, 0.01)
+    sd["actor_critic.action_distribution.linear.bias"] = torch.zeros(4)
+    sd["actor_critic.critic.fc.weight"] = det_uniform((1, 512), seed, 9905, -0.01, 0.01)
+    return {"state_dict": sd, "extra_state": {"step": 0}}
+
+
+def depth_images(n: int, seed: int = 0, height=256, width=256) -> torch.Tensor:
+    """n seeded depth observations (n, height, width, 1) in [0, 1], as habitat delivers observations["depth"]"""
+    return det_uniform((n, height, width, 1), seed, 9999, 0.0, 1.0)
