@@ -300,6 +300,34 @@ int bb_depth_stem(const float* depth, int N, int Hd, int Wd, int64_t sn, int64_t
 int bb_groupnorm_apply(const void* x, const void* stats, int tm, const float* gamma, const float* beta, const void* x2,
                        const void* stats2, int tm2, const float* gamma2, const float* beta2, const void* identity, int N,
                        int H, int W, int C, int groups, float eps, int mode, int out_f32, void* out, void* stream);
+/* The VLN-CE policy's `waypoint` call around its encoders (csrc/ce_step.cu; Policy_ViewSelection_BEV.py:166-321 with
+ * in_train=False, and the trainer's _vp_feature_variable).  Both read only device memory, so they run inside a graph.
+ * bb_ce_view_stack: table (device, 24 entries) holds the k-th rgb view of the observation dict's order at [k] and its
+ * depth partner at [12 + k]; element (b, h, w, c) of a view is at ptr + b*sb + h*sh + w*sw + c*sc (in elements: uint8
+ * rgb (B, rgb_h, rgb_w, 3), f32 depth (B, depth_h, depth_w, 1)).  View k of environment b goes to image
+ * n = (12 - k) % 12 + 12 b of rgb_out (12 B, rgb_h, rgb_w, 3) uint8 and depth_out (12 B, depth_h, depth_w) f32, and
+ * grid_out (12 B, 196) f32 gets the 14 x 14 adaptive average pool of each depth image, bit-identical to the CUDA
+ * AdaptiveAvgPool2d((14, 14)) of the reference.  depth_h, depth_w >= 14; outputs must not overlap.
+ * bb_ce_waypoint_candidates: per environment b, of logits (B, 120, 12) f32, rgb_vec (12 B, 512) and depth_feat (12 B,
+ * 128, 4, 4) f32 in clockwise image order: softmax over the 1440 cells (expf(x - max) / sum), the one-row wrap to
+ * 122 x 12, bb_waypoint_nms's rounds with max_predictions 5 and sigma (7, 5), the wrap rows stripped, and the nonzero
+ * cells in row-major order.  picks (B, BB_CE_PICK_COLS) int32: (angle, distance) pairs in columns 0..9 (0 past the
+ * count), the count K <= 5 in column 10 and the panorama view length K + 12 - |distinct candidate views| in column 11.
+ * prob (B, 120, 12) gets the softmax (may be NULL).  pano_rgb (B, 12, 512) and pano_depth (B, 12, 128) are in
+ * counter-clockwise view order (view 0 stays, 1..11 flipped), pano_depth the 4 x 4 mean; cand_rgb (B, 5, 512) and
+ * cand_depth (B, 5, 128) hold view 12 - (a + 5) / 10 (12 -> 0) of each pick, zeros past K; rgb_fts (B, 17, 512) and
+ * dep_fts (B, 17, 128) hold the candidates, then the views without a candidate in ascending order, then zeros.
+ * Pointers 4-byte aligned; outputs must not overlap each other or the inputs. */
+#define BB_CE_PICK_COLS 12
+typedef struct bb_ce_view {
+  const void* ptr;
+  int64_t sb, sh, sw, sc;
+} bb_ce_view;
+int bb_ce_view_stack(const bb_ce_view* table, int B, int rgb_h, int rgb_w, int depth_h, int depth_w, uint8_t* rgb_out,
+                     float* depth_out, float* grid_out, void* stream);
+int bb_ce_waypoint_candidates(const float* logits, const float* rgb_vec, const float* depth_feat, int B, int* picks,
+                              float* prob, float* pano_rgb, float* pano_depth, float* cand_rgb, float* cand_depth,
+                              float* rgb_fts, float* dep_fts, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

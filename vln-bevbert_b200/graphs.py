@@ -284,11 +284,13 @@ class Surface:
     (`dims`), the model on padded inputs (`padded(model, mode, pad, host)`), the outputs cut back to the caller's
     shapes (`slice(mode, out, batch)`) and the unwrapped call (`eager(model, mode, batch)`).  `grad_ok`: eval-mode
     calls replay with grad enabled too (a frozen, forward-only model); `stale(model)`: True when the weights changed
-    since the previous call, so that every call, not only `language`, re-casts the shadows first."""
+    since the previous call, so that every call, not only `language`, re-casts the shadows first.  `shape_key(mode,
+    batch)`: hashable sizes of a call that its inputs' shapes do not show; they join the bucket key and reach `padded`
+    as `host`."""
 
-    def __init__(self, dims, padded, slice, eager, grad_ok=False, stale=None):
+    def __init__(self, dims, padded, slice, eager, grad_ok=False, stale=None, shape_key=None):
         self.dims, self.padded, self.slice, self.eager = dims, padded, slice, eager
-        self.grad_ok, self.stale = grad_ok, stale
+        self.grad_ok, self.stale, self.shape_key = grad_ok, stale, shape_key
 
 
 NAV = Surface(NAV_PAD_DIMS, nav_forward_padded, nav_slice,
@@ -462,6 +464,71 @@ def install_ce_depth_encoder(depth_encoder):
     return replay
 
 
+# ------------------------------------------------------------ VLN-CE policy `waypoint` call (model/ce_waypoint_step.py)
+# One mode; the only input is the (24, 5) view table, staged on the device before each call.  The geometry (B, rgb and
+# depth image sizes) is the call's shape key.
+CE_STEP_DIMS = {"waypoint": {"views": ()}}
+_WAYPOINT_ARGS = ("mode", "waypoint_predictor", "observations", "in_train")
+
+
+def install_ce_waypoint_step(net):
+    """Makes the CE policy network's `waypoint` call (Policy_ViewSelection_BEV.py BEV.forward with mode='waypoint')
+    one CUDA graph replay: install on `policy.net` (`policy.net.module` under DDP); `net.forward` is replaced.  A call
+    with mode='waypoint' and in_train=False whose observations model.ce_waypoint_step.covered accepts runs
+    model.ce_waypoint_step.WaypointStep over the network's encoders and the call's `waypoint_predictor` (unwrapped
+    from DataParallel; a different predictor module rebuilds the step's graphs), replaying one graph per (B, image
+    sizes) whatever the network's train / eval switch, and returns the reference's output dict (a StepOutputs).  Every
+    other call (other modes, in_train=True, observations not covered) runs the original forward unchanged.  A weight
+    change (load_state_dict) of any of the three modules is seen by the next call.  -> the WaypointStep (its `replay`,
+    a GraphedNavigation, once a call has been replayed)."""
+    import inspect
+    from .model import ce_waypoint_step as CS
+    step = CS.WaypointStep(net)
+    step.replay = None
+    original = net.forward
+    sig = inspect.signature(original)
+
+    def eager(st, mode, batch):                 # a bucket without a graph: the same kernels and the same output dict
+        return st.outputs(st.run(batch["views"], batch["geom"]), batch["geom"][0])
+    surface = Surface(CE_STEP_DIMS, lambda st, mode, pad, host=None: st.run(pad["views"], host),
+                      lambda mode, out, batch: step.outputs(out, batch["geom"][0]), eager,
+                      grad_ok=True, stale=lambda st: st.changed(), shape_key=lambda mode, batch: batch["geom"])
+
+    def forward(*args, **kwargs):
+        bound = sig.bind(*args, **kwargs)
+        bound.apply_defaults()
+        a = bound.arguments
+        if a["mode"] != "waypoint" or a["in_train"] or not isinstance(a["observations"], dict):
+            return original(*args, **kwargs)
+        cov = CS.covered(a["observations"], step.clip.res, step.device)
+        if cov is None:
+            return original(*args, **kwargs)
+        if step.set_predictor(a["waypoint_predictor"]):
+            step.replay = GraphedNavigation(step, surface)
+        step.check_call()
+        pairs, geom = cov
+        table = CS.view_table(a["observations"], pairs).pin_memory().to(step.device, non_blocking=True)
+        return step.replay("waypoint", {"views": table, "geom": geom})
+    net.forward = forward
+    return step
+
+
+def install_ce_vp_features(trainer):
+    """Replaces the CE trainer's `_vp_feature_variable(obs)`: for outputs of an installed waypoint step
+    (install_ce_waypoint_step) it returns the step's padded panorama inputs, sliced to the batch's longest view list,
+    with loc_fts, nav_types and view_lens built on the host and uploaded in one copy; any other dict goes to the
+    trainer's original method."""
+    from .model.ce_waypoint_step import StepOutputs
+    original = trainer._vp_feature_variable
+
+    def vp_feature_variable(obs):
+        if isinstance(obs, StepOutputs):
+            return obs.vp_inputs()
+        return original(obs)
+    trainer._vp_feature_variable = vp_feature_variable
+    return vp_feature_variable
+
+
 class GraphedNavigation:
     """The agents' per-step calls `model(mode, batch)` (GlocalTextPathNavCMT: language / panorama / navigation) replayed
     as CUDA graphs.  Called like the model, with the same inputs and outputs.
@@ -513,7 +580,7 @@ class GraphedNavigation:
             return self._eager(mode, batch)
         if mode == "language" or not self.fresh or (self.s.stale is not None and self.s.stale(self.model)):
             self.refresh()
-        key = _bucket(self.s.dims, mode, batch)
+        key = self._key(mode, batch)
         ent = self.entries.get(key)
         if ent is None:
             ent = self.entries[key] = self._new_entry(mode, batch)
@@ -535,6 +602,10 @@ class GraphedNavigation:
             ent["done"].record()
         return self.s.slice(mode, ent["out"], batch)
 
+    def _key(self, mode, batch):
+        key = _bucket(self.s.dims, mode, batch)
+        return key if self.s.shape_key is None else key + (self.s.shape_key(mode, batch),)
+
     def _new_entry(self, mode, batch):
         dev = self.params[0].device
         bufs = {}
@@ -542,7 +613,7 @@ class GraphedNavigation:
             if k is not None:
                 bufs[name] = torch.zeros(k[0], dtype=k[1], device=dev)
         ent = {"in": bufs, "ext": {}, "graph": None, "out": None, "failed": False, "ptrs": None, "launches": None,
-               "stage": None, "host": None}
+               "stage": None, "host": None if self.s.shape_key is None else self.s.shape_key(mode, batch)}
         if mode == "navigation":
             B, G = bufs["gmap_masks"].shape
             Kc = bufs["bev_cand_idxs"].shape[1]
@@ -585,5 +656,5 @@ class GraphedNavigation:
 
     def launches(self, mode, batch):
         """kernels of libbevbert_b200.so inside the graph of this call's bucket, or None when it runs eagerly."""
-        ent = self.entries.get(_bucket(self.s.dims, mode, batch))
+        ent = self.entries.get(self._key(mode, batch))
         return ent["launches"] if ent is not None and ent["graph"] is not None else None
