@@ -317,7 +317,19 @@ int bb_groupnorm_apply(const void* x, const void* stats, int tm, const float* ga
  * counter-clockwise view order (view 0 stays, 1..11 flipped), pano_depth the 4 x 4 mean; cand_rgb (B, 5, 512) and
  * cand_depth (B, 5, 128) hold view 12 - (a + 5) / 10 (12 -> 0) of each pick, zeros past K; rgb_fts (B, 17, 512) and
  * dep_fts (B, 17, 128) hold the candidates, then the views without a candidate in ascending order, then zeros.
- * Pointers 4-byte aligned; outputs must not overlap each other or the inputs. */
+ * Pointers 4-byte aligned; outputs must not overlap each other or the inputs.
+ * bb_ce_waypoint_candidates_aug: the same call with in_train=True (waypoint augmentation, Policy_ViewSelection_BEV.py:
+ * 229-264).  After the NMS picks (written to nms_picks in the picks layout when it is not NULL), pick k of environment
+ * b at angle a samples from its clockwise image img = (a + 5) / 10 (12 -> 0): the 120 regional logits
+ * logits[b, (10 img + r - 5) mod 120, d] at s = 12 r + d, their softmax, Categorical's renormalisation p / sum(p), and
+ * torch.multinomial's single draw s = argmax(p / q) over the Exp(1) row q = noise[b, k] (noise (B, 5, 120) f32; rows
+ * at or past K are not read), NaN the maximum and the lowest index on ties.  The sampled pick is angle
+ * s / 12 + ((img - 1) * 10 + 5, or 0 for image 0) and distance s % 12; picks holds the sampled pairs, K and the view
+ * length K + 12 - |distinct sampled views|, and every feature output follows the sampled views.  Arithmetic: the
+ * regional softmax is torch 2.11's CUDA softmax for rows of 120 (expf, per-lane sums and a warp butterfly); the
+ * renormalising sum is in this kernel's own order, which was not matched to torch's reduction, then p / sum and p / q
+ * are correctly rounded fp32 divisions.  The reference's random stream is not reproduced: its draws depend on K, which
+ * only the device knows. */
 #define BB_CE_PICK_COLS 12
 typedef struct bb_ce_view {
   const void* ptr;
@@ -328,6 +340,9 @@ int bb_ce_view_stack(const bb_ce_view* table, int B, int rgb_h, int rgb_w, int d
 int bb_ce_waypoint_candidates(const float* logits, const float* rgb_vec, const float* depth_feat, int B, int* picks,
                               float* prob, float* pano_rgb, float* pano_depth, float* cand_rgb, float* cand_depth,
                               float* rgb_fts, float* dep_fts, void* stream);
+int bb_ce_waypoint_candidates_aug(const float* logits, const float* noise, const float* rgb_vec, const float* depth_feat,
+                                  int B, int* picks, int* nms_picks, float* pano_rgb, float* pano_depth,
+                                  float* cand_rgb, float* cand_depth, float* rgb_fts, float* dep_fts, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

@@ -5,8 +5,11 @@
 //     depth grid (AdaptiveAvgPool2d((14, 14)) in the CUDA device's own arithmetic).
 //   bb_ce_waypoint_candidates: heatmap logits -> softmax, one-row wrap, NMS (waypoint_nms.cuh), strip, the nonzero
 //     cells as (angle, distance) picks, and every feature array the `panorama` call takes.
+//   bb_ce_waypoint_candidates_aug: the same with in_train=True (waypoint augmentation, lines 229-264): each pick is
+//     replaced by a cell sampled from its image's regional softmax, given the caller's Exp(1) noise.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include "../../include/bevbert_b200.h"
 #include "common.h"
@@ -90,10 +93,92 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float* red) 
 // the clockwise image of counter-clockwise view j: view 0 stays, views 1..11 are flipped
 __device__ __forceinline__ int cw_image(int j) { return (VIEWS - j) % VIEWS; }
 
-// One CTA per environment b.
+// Writes one environment's picks row (pairs, count, view length) from cnt (angle, distance) pairs, and row_view: the
+// counter-clockwise view of each panorama input row (the candidates' views, then the views without a candidate in
+// ascending order, then -1).
+__device__ void write_picks(int* pk, const int* ang, const int* dist, int cnt, int* row_view) {
+  bool cand_view[VIEWS] = {};
+  for (int q = 0; q < MAX_PRED; ++q) {
+    const int a = q < cnt ? ang[q] : 0, d = q < cnt ? dist[q] : 0;
+    pk[2 * q] = a;
+    pk[2 * q + 1] = d;
+    int img = VIEWS - (a + 5) / 10;
+    if (img == VIEWS) img = 0;
+    if (q < cnt) cand_view[img] = true, row_view[q] = img;
+  }
+  int len = cnt;
+  for (int j = 0; j < VIEWS; ++j)
+    if (!cand_view[j]) row_view[len++] = j;
+  for (int t = len; t < VIEW_ROWS; ++t) row_view[t] = -1;
+  pk[2 * MAX_PRED] = cnt;
+  pk[2 * MAX_PRED + 1] = len;
+}
+
+// Waypoint augmentation of one pick at angle a, by one warp: the 120 regional logits of its clockwise image
+// img = (a + 5) / 10 (12 -> 0), logits[(10 img + r - 5) mod 120, d] at s = 12 r + d; their softmax in the arithmetic of
+// torch's CUDA softmax for rows of 120 (lane l holds s = l + 32 it; a sequential ternary max and sum per lane, then a
+// butterfly); Categorical's renormalisation p / sum(p), the sum in this kernel's own order (per lane, then a
+// butterfly); and torch.multinomial's single draw argmax(p / q) over the noise row q, under torch.argmax's rules.  The
+// sample s becomes angle s / 12 + ((img - 1) * 10 + 5, or 0 for image 0) and distance s % 12.
+__device__ __forceinline__ void sample_pick(const float* __restrict__ x, const float* __restrict__ q, int a, int* ang,
+                                            int* dist) {
+  constexpr int IT = 4, REGION = ANGLES;   // 120 = 10 angles x 12 distances, 4 x 32 lanes
+  const int lane = threadIdx.x & 31;
+  int img = (a + 5) / 10;
+  if (img == VIEWS) img = 0;
+  float e[IT];
+#pragma unroll
+  for (int it = 0; it < IT; ++it) {
+    const int s = lane + 32 * it, r = s / DISTS, d = s - r * DISTS;
+    e[it] = s < REGION ? x[((10 * img + r - 5 + ANGLES) % ANGLES) * DISTS + d] : -__int_as_float(0x7f800000);
+  }
+  float m = e[0];
+#pragma unroll
+  for (int it = 1; it < IT; ++it) m = m > e[it] ? m : e[it];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    m = m < om ? om : m;
+  }
+  float sum = 0.f;
+#pragma unroll
+  for (int it = 0; it < IT; ++it) {
+    e[it] = expf(__fsub_rn(e[it], m));
+    sum = __fadd_rn(sum, e[it]);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, o));
+  float norm = 0.f;
+#pragma unroll
+  for (int it = 0; it < IT; ++it) {
+    e[it] = __fdiv_rn(e[it], sum);
+    if (lane + 32 * it < REGION) norm = __fadd_rn(norm, e[it]);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) norm = __fadd_rn(norm, __shfl_xor_sync(0xffffffffu, norm, o));
+  float bv = -__int_as_float(0x7f800000);
+  int bi = 0x7fffffff;
+#pragma unroll
+  for (int it = 0; it < IT; ++it) {
+    const int s = lane + 32 * it;
+    if (s >= REGION) continue;
+    const float v = __fdiv_rn(__fdiv_rn(e[it], norm), q[s]);
+    if (nms::beats(v, s, bv, bi)) bv = v, bi = s;
+  }
+  nms::warp_best(bv, bi);
+  if (lane == 0) {
+    *ang = bi / DISTS + (img != 0 ? (img - 1) * 10 + 5 : 0);
+    *dist = bi % DISTS;
+  }
+}
+
+// One CTA per environment b.  AUG: in_train=True, `noise` (B, 5, 120) holds pick k's Exp(1) row at [b, k]; picks gets
+// the sampled pairs, nms_picks (may be NULL) the pre-sampling ones, and the features follow the sampled views.
+template <bool AUG>
 __global__ void __launch_bounds__(CAND_THREADS) ce_waypoint_candidates_kernel(
-    const float* __restrict__ logits, const float* __restrict__ rgb_vec, const float* __restrict__ depth_feat,
-    int* __restrict__ picks, float* __restrict__ prob, float* __restrict__ pano_rgb, float* __restrict__ pano_depth,
+    const float* __restrict__ logits, const float* __restrict__ noise, const float* __restrict__ rgb_vec,
+    const float* __restrict__ depth_feat, int* __restrict__ picks, int* __restrict__ nms_picks,
+    float* __restrict__ prob, float* __restrict__ pano_rgb, float* __restrict__ pano_depth,
     float* __restrict__ cand_rgb, float* __restrict__ cand_depth, float* __restrict__ rgb_fts,
     float* __restrict__ dep_fts) {
   __shared__ float heat[WRAP_CELLS];     // the wrapped softmax map, unsuppressed
@@ -103,6 +188,7 @@ __global__ void __launch_bounds__(CAND_THREADS) ce_waypoint_candidates_kernel(
   __shared__ float red[CAND_THREADS / 32];
   __shared__ nms::Scratch<CAND_THREADS> scratch;
   __shared__ int round_pick[MAX_PRED];
+  __shared__ int pick_ang[MAX_PRED], pick_dist[MAX_PRED];
   __shared__ int row_view[VIEW_ROWS];    // counter-clockwise view of each panorama input row, -1: zeros
   pdl_wait();
   pdl_trigger();
@@ -154,23 +240,19 @@ __global__ void __launch_bounds__(CAND_THREADS) ce_waypoint_candidates_kernel(
       cells[at] = ix;
       ++cnt;
     }
-    int* pk = picks + b * BB_CE_PICK_COLS;
-    bool cand_view[VIEWS] = {};
-    for (int q = 0; q < MAX_PRED; ++q) {
-      const int a = q < cnt ? cells[q] / DISTS - 1 : 0, d = q < cnt ? cells[q] % DISTS : 0;
-      pk[2 * q] = a;
-      pk[2 * q + 1] = d;
-      int img = VIEWS - (a + 5) / 10;
-      if (img == VIEWS) img = 0;
-      if (q < cnt) cand_view[img] = true, row_view[q] = img;
-    }
-    int len = cnt;
-    for (int j = 0; j < VIEWS; ++j)
-      if (!cand_view[j]) row_view[len++] = j;
-    for (int t = len; t < VIEW_ROWS; ++t) row_view[t] = -1;
-    pk[2 * MAX_PRED] = cnt;
-    pk[2 * MAX_PRED + 1] = len;
+    for (int q = 0; q < cnt; ++q) pick_ang[q] = cells[q] / DISTS - 1, pick_dist[q] = cells[q] % DISTS;
+    int* out = AUG ? nms_picks : picks;
+    if (out) write_picks(out + b * BB_CE_PICK_COLS, pick_ang, pick_dist, cnt, row_view);
     scratch.pick = cnt;
+  }
+  if (AUG) {
+    __syncthreads();
+    const int warp = tid >> 5;
+    if (warp < scratch.pick)
+      sample_pick(x, noise + ((long long)b * MAX_PRED + warp) * ANGLES, pick_ang[warp], &pick_ang[warp],
+                  &pick_dist[warp]);
+    __syncthreads();
+    if (tid == 0) write_picks(picks + b * BB_CE_PICK_COLS, pick_ang, pick_dist, scratch.pick, row_view);
   }
   // 6. features.  pano_depth: torch's CUDA mean over the 4 x 4 cells as the device computes it (confirmed on order-
   // sensitive inputs): each cell from +0, a halving tree (cell q += cell q + 8, then + 4, + 2, + 1), then times 1/16.
@@ -252,35 +334,84 @@ extern "C" int bb_ce_view_stack(const bb_ce_view* table, int B, int rgb_h, int r
   return check_launch("ce_view_stack_kernel");
 }
 
-extern "C" int bb_ce_waypoint_candidates(const float* logits, const float* rgb_vec, const float* depth_feat, int B,
-                                         int* picks, float* prob, float* pano_rgb, float* pano_depth, float* cand_rgb,
-                                         float* cand_depth, float* rgb_fts, float* dep_fts, void* stream) {
-  if (B <= 0 || B > 65535) return set_error("bb_ce_waypoint_candidates: B must be in [1, 65535]");
+namespace bb {
+namespace {
+// The argument checks of both candidate entry points: NULL, alignment, and no output overlapping another output or an
+// input.  noise (AUG only) and the optional prob / nms_picks join the lists when given.
+int check_candidates(const char* name, const float* logits, const float* noise, const float* rgb_vec,
+                     const float* depth_feat, int B, int* picks, int* nms_picks, float* prob, float* pano_rgb,
+                     float* pano_depth, float* cand_rgb, float* cand_depth, float* rgb_fts, float* dep_fts, bool aug) {
+  char msg[160];
+  if (B <= 0 || B > 65535) {
+    snprintf(msg, sizeof msg, "%s: B must be in [1, 65535]", name);
+    return set_error(msg);
+  }
   const void* ptrs[] = {logits, rgb_vec, depth_feat, picks, pano_rgb, pano_depth, cand_rgb, cand_depth, rgb_fts,
-                        dep_fts};
+                        dep_fts, aug ? (const void*)noise : (const void*)logits};
   for (const void* p : ptrs)
-    if (!p) return set_error("bb_ce_waypoint_candidates: only prob may be NULL");
+    if (!p) {
+      snprintf(msg, sizeof msg, "%s: only %s may be NULL", name, aug ? "nms_picks" : "prob");
+      return set_error(msg);
+    }
   for (const void* p : ptrs)
-    if ((uintptr_t)p & 3) return set_error("bb_ce_waypoint_candidates: pointers must be 4-byte aligned");
-  if ((uintptr_t)prob & 3) return set_error("bb_ce_waypoint_candidates: pointers must be 4-byte aligned");
+    if ((uintptr_t)p & 3) {
+      snprintf(msg, sizeof msg, "%s: pointers must be 4-byte aligned", name);
+      return set_error(msg);
+    }
+  if (((uintptr_t)prob & 3) || ((uintptr_t)nms_picks & 3)) {
+    snprintf(msg, sizeof msg, "%s: pointers must be 4-byte aligned", name);
+    return set_error(msg);
+  }
   const long long f = 4LL * B;
   const struct { const void* p; long long n; } outs[] = {
-      {picks, f * BB_CE_PICK_COLS}, {prob, prob ? f * CELLS : 0}, {pano_rgb, f * VIEWS * RGB_DIM},
-      {pano_depth, f * VIEWS * DEP_DIM}, {cand_rgb, f * MAX_PRED * RGB_DIM}, {cand_depth, f * MAX_PRED * DEP_DIM},
-      {rgb_fts, f * VIEW_ROWS * RGB_DIM}, {dep_fts, f * VIEW_ROWS * DEP_DIM}};
-  const struct { const void* p; long long n; } ins[] = {
-      {logits, f * CELLS}, {rgb_vec, f * VIEWS * RGB_DIM}, {depth_feat, f * VIEWS * DEP_DIM * DEP_HW}};
+      {picks, f * BB_CE_PICK_COLS}, {prob, prob ? f * CELLS : 0}, {nms_picks, nms_picks ? f * BB_CE_PICK_COLS : 0},
+      {pano_rgb, f * VIEWS * RGB_DIM}, {pano_depth, f * VIEWS * DEP_DIM}, {cand_rgb, f * MAX_PRED * RGB_DIM},
+      {cand_depth, f * MAX_PRED * DEP_DIM}, {rgb_fts, f * VIEW_ROWS * RGB_DIM}, {dep_fts, f * VIEW_ROWS * DEP_DIM}};
+  const struct { const void* p; long long n; } ins[] = {{logits, f * CELLS},
+                                                        {rgb_vec, f * VIEWS * RGB_DIM},
+                                                        {depth_feat, f * VIEWS * DEP_DIM * DEP_HW},
+                                                        {noise, aug ? f * MAX_PRED * ANGLES : 0}};
   const int n_out = (int)(sizeof(outs) / sizeof(outs[0])), n_in = (int)(sizeof(ins) / sizeof(ins[0]));
   for (int i = 0; i < n_out; ++i) {
     for (int j = i + 1; j < n_out; ++j)
-      if (overlaps(outs[i].p, outs[i].n, outs[j].p, outs[j].n))
-        return set_error("bb_ce_waypoint_candidates: the outputs must not overlap");
+      if (overlaps(outs[i].p, outs[i].n, outs[j].p, outs[j].n)) {
+        snprintf(msg, sizeof msg, "%s: the outputs must not overlap", name);
+        return set_error(msg);
+      }
     for (int j = 0; j < n_in; ++j)
-      if (overlaps(outs[i].p, outs[i].n, ins[j].p, ins[j].n))
-        return set_error("bb_ce_waypoint_candidates: an output overlaps an input");
+      if (overlaps(outs[i].p, outs[i].n, ins[j].p, ins[j].n)) {
+        snprintf(msg, sizeof msg, "%s: an output overlaps an input", name);
+        return set_error(msg);
+      }
   }
-  launch_pdl(ce_waypoint_candidates_kernel, dim3((unsigned)B), dim3(CAND_THREADS), 0, (cudaStream_t)stream, logits,
-             rgb_vec, depth_feat, picks, prob, pano_rgb, pano_depth, cand_rgb, cand_depth, rgb_fts, dep_fts);
+  return 0;
+}
+}  // namespace
+}  // namespace bb
+
+extern "C" int bb_ce_waypoint_candidates(const float* logits, const float* rgb_vec, const float* depth_feat, int B,
+                                         int* picks, float* prob, float* pano_rgb, float* pano_depth, float* cand_rgb,
+                                         float* cand_depth, float* rgb_fts, float* dep_fts, void* stream) {
+  if (check_candidates("bb_ce_waypoint_candidates", logits, nullptr, rgb_vec, depth_feat, B, picks, nullptr, prob,
+                       pano_rgb, pano_depth, cand_rgb, cand_depth, rgb_fts, dep_fts, false))
+    return -1;
+  launch_pdl(ce_waypoint_candidates_kernel<false>, dim3((unsigned)B), dim3(CAND_THREADS), 0, (cudaStream_t)stream,
+             logits, (const float*)nullptr, rgb_vec, depth_feat, picks, (int*)nullptr, prob, pano_rgb, pano_depth,
+             cand_rgb, cand_depth, rgb_fts, dep_fts);
   count_launch();
   return check_launch("ce_waypoint_candidates_kernel");
+}
+
+extern "C" int bb_ce_waypoint_candidates_aug(const float* logits, const float* noise, const float* rgb_vec,
+                                             const float* depth_feat, int B, int* picks, int* nms_picks,
+                                             float* pano_rgb, float* pano_depth, float* cand_rgb, float* cand_depth,
+                                             float* rgb_fts, float* dep_fts, void* stream) {
+  if (check_candidates("bb_ce_waypoint_candidates_aug", logits, noise, rgb_vec, depth_feat, B, picks, nms_picks,
+                       nullptr, pano_rgb, pano_depth, cand_rgb, cand_depth, rgb_fts, dep_fts, true))
+    return -1;
+  launch_pdl(ce_waypoint_candidates_kernel<true>, dim3((unsigned)B), dim3(CAND_THREADS), 0, (cudaStream_t)stream,
+             logits, noise, rgb_vec, depth_feat, picks, nms_picks, (float*)nullptr, pano_rgb, pano_depth, cand_rgb,
+             cand_depth, rgb_fts, dep_fts);
+  count_launch();
+  return check_launch("ce_waypoint_candidates_aug_kernel");
 }

@@ -466,19 +466,22 @@ def install_ce_depth_encoder(depth_encoder):
 
 # ------------------------------------------------------------ VLN-CE policy `waypoint` call (model/ce_waypoint_step.py)
 # One mode; the only input is the (24, 5) view table, staged on the device before each call.  The geometry (B, rgb and
-# depth image sizes) is the call's shape key.
+# depth image sizes) and in_train are the call's shape key, so training and eval rollouts keep a graph each.
 CE_STEP_DIMS = {"waypoint": {"views": ()}}
 _WAYPOINT_ARGS = ("mode", "waypoint_predictor", "observations", "in_train")
 
 
-def install_ce_waypoint_step(net):
+def install_ce_waypoint_step(net, waypoint_aug=False):
     """Makes the CE policy network's `waypoint` call (Policy_ViewSelection_BEV.py BEV.forward with mode='waypoint')
     one CUDA graph replay: install on `policy.net` (`policy.net.module` under DDP); `net.forward` is replaced.  A call
     with mode='waypoint' and in_train=False whose observations model.ce_waypoint_step.covered accepts runs
     model.ce_waypoint_step.WaypointStep over the network's encoders and the call's `waypoint_predictor` (unwrapped
     from DataParallel; a different predictor module rebuilds the step's graphs), replaying one graph per (B, image
-    sizes) whatever the network's train / eval switch, and returns the reference's output dict (a StepOutputs).  Every
-    other call (other modes, in_train=True, observations not covered) runs the original forward unchanged.  A weight
+    sizes, in_train) whatever the network's train / eval switch, and returns the reference's output dict (a
+    StepOutputs).  With waypoint_aug=True, covered in_train=True calls (the trainer's IL.waypoint_aug rollouts) are the
+    step's too: each replay draws fresh Exp(1) noise from torch's default CUDA generator and samples every candidate
+    from it, with the reference's distribution and algorithm but not its random stream.  Every other call (other
+    modes, in_train=True unless waypoint_aug, observations not covered) runs the original forward unchanged.  A weight
     change (load_state_dict) of any of the three modules is seen by the next call.  -> the WaypointStep (its `replay`,
     a GraphedNavigation, once a call has been replayed)."""
     import inspect
@@ -488,17 +491,20 @@ def install_ce_waypoint_step(net):
     original = net.forward
     sig = inspect.signature(original)
 
+    # the shape key (B, Hr, Wr, Hd, Wd, in_train) reaches `padded` as `host`
     def eager(st, mode, batch):                 # a bucket without a graph: the same kernels and the same output dict
-        return st.outputs(st.run(batch["views"], batch["geom"]), batch["geom"][0])
-    surface = Surface(CE_STEP_DIMS, lambda st, mode, pad, host=None: st.run(pad["views"], host),
+        return st.outputs(st.run(batch["views"], batch["geom"], batch["in_train"]), batch["geom"][0])
+    surface = Surface(CE_STEP_DIMS, lambda st, mode, pad, host=None: st.run(pad["views"], host[:5], host[5]),
                       lambda mode, out, batch: step.outputs(out, batch["geom"][0]), eager,
-                      grad_ok=True, stale=lambda st: st.changed(), shape_key=lambda mode, batch: batch["geom"])
+                      grad_ok=True, stale=lambda st: st.changed(),
+                      shape_key=lambda mode, batch: batch["geom"] + (batch["in_train"],))
 
     def forward(*args, **kwargs):
         bound = sig.bind(*args, **kwargs)
         bound.apply_defaults()
         a = bound.arguments
-        if a["mode"] != "waypoint" or a["in_train"] or not isinstance(a["observations"], dict):
+        if (a["mode"] != "waypoint" or (a["in_train"] and not waypoint_aug)
+                or not isinstance(a["observations"], dict)):
             return original(*args, **kwargs)
         cov = CS.covered(a["observations"], step.clip.res, step.device)
         if cov is None:
@@ -508,7 +514,7 @@ def install_ce_waypoint_step(net):
         step.check_call()
         pairs, geom = cov
         table = CS.view_table(a["observations"], pairs).pin_memory().to(step.device, non_blocking=True)
-        return step.replay("waypoint", {"views": table, "geom": geom})
+        return step.replay("waypoint", {"views": table, "geom": geom, "in_train": bool(a["in_train"])})
     net.forward = forward
     return step
 

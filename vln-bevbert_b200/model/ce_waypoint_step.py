@@ -12,6 +12,10 @@ sizes); the observation tensors reach the graph through a 24-entry table of poin
 before each replay.  After the replay one device-to-host copy of the picks (B, 12) int32 feeds the host-side
 outputs, which use the reference's own expressions on the copied indices (`host_outputs`).
 
+With in_train=True (waypoint augmentation, lines 229-264; graphs.install_ce_waypoint_step(net, waypoint_aug=True)) the
+call draws Exp(1) noise inside the graph and bb_ce_waypoint_candidates_aug replaces each NMS pick by a sample of its
+image's regional softmax, the draw torch.multinomial makes for the reference's Categorical(...).sample().
+
 Autocast is disabled inside the call (as in the towers), so the trainer's autocast() changes no bit.  The step runs
 forward only: a call with grad enabled while an encoder or predictor parameter requires grad raises, and so does a call
 while the predictor is in training mode (the reference applies dropout there).
@@ -56,23 +60,31 @@ def view_stack(table, B, rgb_hw, depth_hw, device):
     return rgb, depth, grid
 
 
-def waypoint_candidates(logits, rgb_vec, depth_feats, prob=False):
-    """bb_ce_waypoint_candidates: logits (B, 120, 12), rgb_vec (12 B, 512) and depth_feats (12 B, 128, 4, 4), fp32 CUDA,
-    images in clockwise order -> dict of fresh tensors: picks (B, 12) int32 (pairs, count, view length), pano_rgb,
-    pano_depth, cand_rgb, cand_depth, rgb_fts, dep_fts, and with prob=True the softmax (B, 120, 12)."""
+def _candidate_outputs(logits, rgb_vec, depth_feats, noise=None):
+    """checks the candidate kernels' inputs -> (B, dict of their fresh outputs)"""
     B = logits.shape[0] if logits.dim() == 3 else 0
     want = {"logits": (logits, (B, NUM_ANGLES, NUM_CLASSES)), "rgb_vec": (rgb_vec, (B * NUM_IMGS, RGB_DIM)),
             "depth_feats": (depth_feats, (B * NUM_IMGS, DEP_DIM, 4, 4))}
+    if noise is not None:
+        want["noise"] = (noise, (B, MAX_PRED, NUM_ANGLES))
     for name, (t, shape) in want.items():
         if t.dtype != torch.float32 or not t.is_cuda:
             raise TypeError("%s must be a float32 CUDA tensor, got %s on %s" % (name, t.dtype, t.device))
         if B == 0 or tuple(t.shape) != shape or not t.is_contiguous():
             raise ValueError("%s must be contiguous %s, got %s" % (name, shape, tuple(t.shape)))
     f = dict(dtype=torch.float32, device=logits.device)
-    out = {"picks": torch.empty(B, PICK_COLS, dtype=torch.int32, device=logits.device),
-           "pano_rgb": torch.empty(B, NUM_IMGS, RGB_DIM, **f), "pano_depth": torch.empty(B, NUM_IMGS, DEP_DIM, **f),
-           "cand_rgb": torch.empty(B, MAX_PRED, RGB_DIM, **f), "cand_depth": torch.empty(B, MAX_PRED, DEP_DIM, **f),
-           "rgb_fts": torch.empty(B, VIEW_ROWS, RGB_DIM, **f), "dep_fts": torch.empty(B, VIEW_ROWS, DEP_DIM, **f)}
+    return B, {"picks": torch.empty(B, PICK_COLS, dtype=torch.int32, device=logits.device),
+               "pano_rgb": torch.empty(B, NUM_IMGS, RGB_DIM, **f), "pano_depth": torch.empty(B, NUM_IMGS, DEP_DIM, **f),
+               "cand_rgb": torch.empty(B, MAX_PRED, RGB_DIM, **f), "cand_depth": torch.empty(B, MAX_PRED, DEP_DIM, **f),
+               "rgb_fts": torch.empty(B, VIEW_ROWS, RGB_DIM, **f), "dep_fts": torch.empty(B, VIEW_ROWS, DEP_DIM, **f)}
+
+
+def waypoint_candidates(logits, rgb_vec, depth_feats, prob=False):
+    """bb_ce_waypoint_candidates: logits (B, 120, 12), rgb_vec (12 B, 512) and depth_feats (12 B, 128, 4, 4), fp32 CUDA,
+    images in clockwise order -> dict of fresh tensors: picks (B, 12) int32 (pairs, count, view length), pano_rgb,
+    pano_depth, cand_rgb, cand_depth, rgb_fts, dep_fts, and with prob=True the softmax (B, 120, 12)."""
+    B, out = _candidate_outputs(logits, rgb_vec, depth_feats)
+    f = dict(dtype=torch.float32, device=logits.device)
     if prob:
         out["prob"] = torch.empty(B, NUM_ANGLES, NUM_CLASSES, **f)
     o = out
@@ -82,6 +94,29 @@ def waypoint_candidates(logits, rgb_vec, depth_feats, prob=False):
         o["cand_rgb"].data_ptr(), o["cand_depth"].data_ptr(), o["rgb_fts"].data_ptr(), o["dep_fts"].data_ptr(),
         K._stream()), "bb_ce_waypoint_candidates")
     return out
+
+
+def waypoint_candidates_aug(logits, noise, rgb_vec, depth_feats, nms_picks=False):
+    """bb_ce_waypoint_candidates_aug (in_train=True): as waypoint_candidates, with each NMS pick k of environment b
+    replaced by the cell sampled from its image's regional softmax under the Exp(1) noise row noise[b, k] (noise
+    (B, 5, 120) fp32 CUDA).  picks and the features follow the sampled cells; with nms_picks=True the dict also holds
+    the pre-sampling picks (B, 12) int32 as "nms_picks"."""
+    B, out = _candidate_outputs(logits, rgb_vec, depth_feats, noise)
+    if nms_picks:
+        out["nms_picks"] = torch.empty(B, PICK_COLS, dtype=torch.int32, device=logits.device)
+    o = out
+    _lib.check(_lib.load().bb_ce_waypoint_candidates_aug(
+        logits.data_ptr(), noise.data_ptr(), rgb_vec.data_ptr(), depth_feats.data_ptr(), B, o["picks"].data_ptr(),
+        o["nms_picks"].data_ptr() if nms_picks else None, o["pano_rgb"].data_ptr(), o["pano_depth"].data_ptr(),
+        o["cand_rgb"].data_ptr(), o["cand_depth"].data_ptr(), o["rgb_fts"].data_ptr(), o["dep_fts"].data_ptr(),
+        K._stream()), "bb_ce_waypoint_candidates_aug")
+    return out
+
+
+def draw_noise(B, device):
+    """the Exp(1) noise of one in_train=True call, (B, 5, 120) fp32, from torch's default generator of `device` on the
+    current stream: torch.multinomial's single draw is argmax(p / q) with q = empty_like(p).exponential_(1)"""
+    return torch.empty(B, MAX_PRED, NUM_ANGLES, dtype=torch.float32, device=device).exponential_(1)
 
 
 # ------------------------------------------------------------------------------------------------- host logic
@@ -180,9 +215,10 @@ def vp_host_inputs(obs):
 
 class StepOutputs(dict):
     """The reference's `waypoint` output dict (same keys, value types, devices and dtypes), computed by the step.  It
-    also carries the step's picks (B, 12) int32 on the host (`picks`) and the padded panorama inputs of the same replay
+    also carries the step's picks (B, 12) int32 on the host (`picks`), the padded panorama inputs of the same replay
     (`padded`), which graphs.install_ce_vp_features hands to the
-    `panorama` call in place of _vp_feature_variable's per-environment concatenations."""
+    `panorama` call in place of _vp_feature_variable's per-environment concatenations, and for an in_train=True call
+    the (B, 5, 120) Exp(1) noise its candidates were sampled with (`noise`, else None)."""
 
     def vp_inputs(self):
         """_vp_feature_variable(self): rgb_fts, dep_fts (device, sliced to the longest view list), loc_fts, nav_types
@@ -253,21 +289,30 @@ class WaypointStep:
         self.depth.check_grad()
         self.runner.check_call()
 
-    def run(self, table, geom):
-        """the call on a staged view table (24, 5) and its geometry (B, Hr, Wr, Hd, Wd) -> dict of device tensors"""
+    def run(self, table, geom, in_train=False):
+        """the call on a staged view table (24, 5) and its geometry (B, Hr, Wr, Hd, Wd) -> dict of device tensors.
+        in_train=True draws the call's noise (draw_noise; inside a graph every replay draws afresh) and samples the
+        candidates from it; the noise is returned as "noise"."""
         B, Hr, Wr, Hd, Wd = geom
         with torch.autocast("cuda", enabled=False), torch.no_grad():
             rgb, depth, grid = view_stack(table, B, (Hr, Wr), (Hd, Wd), self.device)
             depth_feats = self.depth._encode(depth)
             rgb_vec, rgb_grid = self.clip._encode(rgb, self.clip.mean, self.clip.std)
             logits = self.runner._forward(depth_feats, B)
-            out = waypoint_candidates(logits, rgb_vec, depth_feats.contiguous())
+            if in_train:
+                noise = draw_noise(B, self.device)
+                out = waypoint_candidates_aug(logits, noise, rgb_vec, depth_feats.contiguous())
+                out["noise"] = noise
+            else:
+                out = waypoint_candidates(logits, rgb_vec, depth_feats.contiguous())
         out.update(rgb_grid=rgb_grid, depth_grid=grid)
         return out
 
     def outputs(self, out, B):
         """the reference's output dict from the step's device outputs `out`; the copy of the picks is the call's one
-        host synchronisation"""
+        host synchronisation.  For an in_train=True call (`out` holds "noise") the reference's sampled index tensors
+        are CPU tensors (torch.tensor over a list of 0-d tensors), so the angles divide on the CPU, and the result
+        carries a copy of the noise as `noise`."""
         c = torch.Tensor.clone
         cand_rgb, cand_depth = c(out["cand_rgb"]), c(out["cand_depth"])
         res = {"pano_rgb": c(out["pano_rgb"]), "pano_depth": c(out["pano_depth"]),
@@ -276,7 +321,7 @@ class WaypointStep:
         picks = out["picks"].cpu()
         L = int(picks[:, 2 * MAX_PRED + 1].max())
         padded = (c(out["rgb_fts"][:, :L]), c(out["dep_fts"][:, :L]))
-        host = host_outputs(picks, self.device.type)
+        host = host_outputs(picks, "cpu" if "noise" in out else self.device.type)
         counts = picks[:, 2 * MAX_PRED].tolist()
         o = StepOutputs(cand_rgb=[cand_rgb[j, :k] for j, k in enumerate(counts)],
                         cand_depth=[cand_depth[j, :k] for j, k in enumerate(counts)],
@@ -287,4 +332,5 @@ class WaypointStep:
                         pano_angle_fts=copy.deepcopy(self.net.pano_angle_fts),
                         pano_img_idxes=copy.deepcopy(self.net.pano_img_idxes))
         o.padded, o.picks = padded, picks
+        o.noise = c(out["noise"]) if "noise" in out else None
         return o
