@@ -343,6 +343,23 @@ int bb_ce_waypoint_candidates(const float* logits, const float* rgb_vec, const f
 int bb_ce_waypoint_candidates_aug(const float* logits, const float* noise, const float* rgb_vec, const float* depth_feat,
                                   int B, int* picks, int* nms_picks, float* pano_rgb, float* pano_depth,
                                   float* cand_rgb, float* cand_depth, float* rgb_fts, float* dep_fts, void* stream);
+/* The VLN-CE trainer's gmap_img_fts (ss_trainer_BEV.py:1032-1033, 1060-1066, 534-611 with graph_utils.py:198-281) from
+ * the episode's stored `panorama` outputs, one launch per `navigation` call; the int32 table lives on the device.
+ * Table: S step records of BB_CE_GMAP_STEP_WORDS words (pointer words as lo, hi: pano_embeds (Bs, Vs, H) f32, nav_types
+ * (Bs, Vs) int64, pano_masks (Bs, Vs) bool, then Bs, Vs), then B * G row records (kind, a, c), then term records
+ * (s, i, k).  Row kind 0: zeros (row 0 and padding).  Kind 1, node (a = step, c = row): the masked mean of
+ * pano[a][c], in torch 2.11's CUDA arithmetic of sum(pano * mask, 1) / sum(mask, 1) for Vs < 64 (four accumulators
+ * from +0 over views v = j mod 4, ascending, then ((a0 + a1) + a2) + a3, then a correctly rounded division by the
+ * count).  Kind 2, ghost: terms a .. a + c - 1, each the k-th candidate (nav_types == 1, ascending) of pano[s][i],
+ * summed left to right in merge order, then times the fp32 reciprocal of c, as torch divides a CUDA tensor by a Python
+ * number; a term whose row has no k-th candidate gives NaN.  out (B, G, H) f32, H a multiple of 4, 16-byte aligned.
+ * bb_ce_gmap_features_bwd: the same step records with the gradient buffers of pano_embeds in place of pano_embeds
+ * (every row written), then R records (s, i, node b, node r or b = -1, first candidate record, candidate count), then
+ * candidate records (ghost b or -1, ghost r, ghost count) in k order.  d pano[s][i][v] = dout[node] / sum(mask) where
+ * mask[v], plus dout[ghost] * fp32(1 / count) where v is a merged candidate, added in that order; +0 otherwise. */
+#define BB_CE_GMAP_STEP_WORDS 8
+int bb_ce_gmap_features(const int32_t* table, int S, int B, int G, int H, float* out, void* stream);
+int bb_ce_gmap_features_bwd(const int32_t* table, int S, int R, int Vmax, int G, int H, const float* dout, void* stream);
 /* in-place x[r,:] *= g[r] on a bf16 (rows, ld) matrix. */
 int bb_scale_rows_bf16(void* x, const float* g, int64_t rows, int64_t ld, void* stream);
 /* Segment weighted sum (vilmodel.py:632-666 _aggregate_gmap_features, host loops turned into CSR lists):

@@ -151,6 +151,8 @@ _SIGNATURES = {
     "bb_ce_view_stack": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "bb_ce_waypoint_candidates": (c_int, [c_void_p, c_void_p, c_void_p, c_int] + [c_void_p] * 8 + [c_void_p]),
     "bb_ce_waypoint_candidates_aug": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 8 + [c_void_p]),
+    "bb_ce_gmap_features": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "bb_ce_gmap_features_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "bb_scale_rows_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p]),
     "bb_segment_wsum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),
     "bb_segment_wsum_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p]),

@@ -22,8 +22,10 @@ gradients); a step whose capture fails (a host synchronisation somewhere in forw
 `GraphedNavigation` (below) replays the agents' per-step inference calls the same way, over padded shape buckets,
 `install_ce_replay` the VLN-CE policy's, `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder,
 `install_ce_depth_encoder` its ResNet-50 depth encoder, and `install_ce_waypoint_predictor` the CE trainer's waypoint
-predictor.
+predictor.  `install_ce_gmap_features` builds the CE trainer's global-map image input on the kernels (no replay).
 """
+import functools
+
 import torch
 
 from . import blocks
@@ -533,6 +535,43 @@ def install_ce_vp_features(trainer):
         return original(obs)
     trainer._vp_feature_variable = vp_feature_variable
     return vp_feature_variable
+
+
+def install_ce_gmap_features(trainer):
+    """Builds the CE trainer's `gmap_img_fts` on the kernels (ce_gmap.py) instead of the rollout's per-environment
+    tensor glue.  On the trainer's instances only:
+      * `trainer.policy.net`'s `panorama` calls record their outputs (pano_embeds, the call's nav_types, pano_masks) in
+        the episode's ce_gmap.Memory, which starts when the call first sees a fresh `trainer.gmaps`;
+      * each of those GraphMaps gets an `update_graph` that replaces the embedding arguments the rollout passes with
+        handles to the step's rows (ghost merges add handles, in merge order) before running the original, and a
+        `get_node_embeds` that returns the row the kernel computes, so other callers keep working;
+      * `trainer._nav_gmap_variable` runs the trainer's own method for every other key and returns `gmap_img_fts`
+        from one bb_ce_gmap_features launch, differentiable with respect to every stored step's pano_embeds.
+    Nothing in it synchronises with the host.  The rollout's own masked mean and boolean index still run, and their
+    results are no longer read.  -> the installed _nav_gmap_variable."""
+    from . import ce_gmap
+    net, original = trainer.policy.net, trainer._nav_gmap_variable
+    forward = net.forward
+
+    @functools.wraps(forward)       # keeps the signature, which install_ce_waypoint_step binds, if installed after this
+    def panorama_forward(*args, **kwargs):
+        out = forward(*args, **kwargs)
+        if kwargs.get("mode") == "panorama":
+            mem = ce_gmap.episode(trainer.gmaps)
+            if mem is None:
+                mem = ce_gmap.Memory()
+                for g in trainer.gmaps:
+                    ce_gmap.attach(trainer, g, mem)
+            mem.record(out[0], kwargs["nav_types"], out[1])
+        return out
+
+    def nav_gmap_variable(cur_vp, cur_pos, cur_ori):
+        out, rows = ce_gmap.trainer_method(original, trainer.gmaps, cur_vp, cur_pos, cur_ori)
+        out["gmap_img_fts"] = ce_gmap.episode(trainer.gmaps).features(rows)
+        return out
+    net.forward = panorama_forward
+    trainer._nav_gmap_variable = nav_gmap_variable
+    return nav_gmap_variable
 
 
 class GraphedNavigation:
