@@ -121,6 +121,16 @@ int bb_bev_lift_index(const float* depths, const float* T_c2w, const float* S_w2
                       int Hf, int Wf, float depth_scale, float fx, float fy, float cx, float cy, int map_dim,
                       float map_res, float y_clip, int32_t* cell_idx, float* pc_out, void* stream);
 
+/* World points of N depth views (PointCloud.forward, bev_utils.py:349-378, as the VLN-CE trainer's `lift` calls it,
+ * ss_trainer_BEV.py:386-410): depths f32 (N, Hf, Wf) stored units (z = depth * depth_scale); T_c2w f32 (N, 4, 4) row
+ * major; world_shift f32 (3) on the device (world_shift_origin).  pts f32 (N*Hf*Wf, 3) = T * (x, y, z, 1) - world_shift
+ * with x = z * ((col + 0.5 - cx) / fx), y = z * ((row + 0.5 - cy) / fy), each row of T dotted left to right in
+ * round-to-nearest single operations, the arithmetic of bb_bev_lift_index's world point; no_depth u8 (N*Hf*Wf) =
+ * (z == 0).  Float pointers 4-byte aligned; N > 0 and Hf * Wf within int32. */
+int bb_bev_lift_points(const float* depths, const float* T_c2w, int N, int Hf, int Wf, float depth_scale, float fx,
+                       float fy, float cx, float cy, const float* world_shift, float* pts, uint8_t* no_depth,
+                       void* stream);
+
 /* Cell index of a ready-made ego-frame point cloud (PointCloud.project_bev, pretrain_src/model/bev_utils.py:381-406,
  * map_nav_src/models/bev_utils.py:382-401): pc f32 (npoints, 3), no_depth u8 (npoints) or NULL -> cell_idx int32
  * (npoints): D*round(z/res + (D-1)/2) + round(x/res + (D-1)/2) (round half to even), -1 when the point has no depth,

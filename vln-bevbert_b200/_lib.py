@@ -108,6 +108,7 @@ _SIGNATURES = {
     "bb_gemm_profile_read": (c_int, [c_i64, C.POINTER(c_float), C.POINTER(c_i64)]),
     "bb_bev_lift_index": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float] * 5 + [c_int, c_float, c_float, c_void_p,
                                                                                   c_void_p, c_void_p]),
+    "bb_bev_lift_points": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_float] * 5 + [c_void_p] * 4),
     "bb_bev_cell_index": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_float, c_float, c_void_p, c_void_p]),
     "bb_bev_scatter_mean_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int] + [c_void_p] * 5),
     "bb_bev_scatter_mean_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int] + [c_void_p] * 5),

@@ -16,6 +16,7 @@ Install on an agent once it is built:
 (bevbert_ce/vlnce_baselines/ss_trainer_BEV.py:477-532); see its docstring.
 """
 import importlib
+import math
 import sys
 
 import numpy as np
@@ -44,16 +45,25 @@ def ego_frames(obs):
     return heading_frames(S, np.array([o["heading"] for o in obs], dtype=np.float64))
 
 
+def frames64(xyzhe):
+    """transfrom3D (bev_utils.py:7-37 of both trees) before its rounding to float32: (N,5) float64 x, y, z, heading,
+    elevation -> (N,4,4) float64 matrices, every entry the same float64 expression as there."""
+    cx, sx = np.cos(xyzhe[:, 4]), np.sin(xyzhe[:, 4])
+    cy, sy = np.cos(xyzhe[:, 3]), np.sin(xyzhe[:, 3])
+    T = np.zeros((len(xyzhe), 4, 4), dtype=np.float64)
+    T[:, 0, 0], T[:, 0, 1], T[:, 0, 2], T[:, 0, 3] = cy, sx * sy, cx * sy, xyzhe[:, 0]
+    T[:, 1, 1], T[:, 1, 2], T[:, 1, 3] = cx, -sx, xyzhe[:, 1]
+    T[:, 2, 0], T[:, 2, 1], T[:, 2, 2], T[:, 2, 3] = -sy, cy * sx, cy * cx, xyzhe[:, 2]
+    T[:, 3, 3] = 1.0
+    return T
+
+
 def heading_frames(S, h):
     """(S, T) float32 from float64 positions S (B,3) and headings h (B,): T rotates about the vertical axis by h
-    (transfrom3D at zero elevation and translation, bev_utils.py:7-37 of both trees)."""
-    c, s = np.cos(h), np.sin(h)
-    T = np.zeros((len(h), 4, 4), dtype=np.float64)
-    T[:, 0, 0], T[:, 0, 2] = c, s
-    T[:, 1, 1] = 1.0
-    T[:, 2, 0], T[:, 2, 2] = -s, c
-    T[:, 3, 3] = 1.0
-    return S.astype(np.float32), T.astype(np.float32)
+    (transfrom3D at zero elevation and translation)."""
+    xyzhe = np.zeros((len(h), 5), dtype=np.float64)
+    xyzhe[:, 3] = h
+    return S.astype(np.float32), frames64(xyzhe).astype(np.float32)
 
 
 def nav_bev_variable(agent, obs, gmaps):
@@ -101,6 +111,72 @@ def _trainer_heading_fn(trainer):
         if fn is not None:
             return fn
     return importlib.import_module("vlnce_baselines.models.graph_utils").heading_from_quaternion
+
+
+LIFT_VIEWS, LIFT_GRID, LIFT_DIM = 12, 14, 768       # lift's views, depth-grid side and feature width (:389,402,407)
+
+
+def lift_frames(cur_pos, headings):
+    """`lift`'s camera-to-world fan (ss_trainer_BEV.py:391-399): per environment the 12 views at headings
+    -arange(12) * radians(30) + heading, elevation pi and translation (x, y, z), built in float64 as there and rounded
+    to float32 like transfrom3D -> (B * 12, 4, 4) float32.  `headings[i]`: heading_from_quaternion(cur_ori[i])."""
+    xyzhe = np.zeros([len(cur_pos), LIFT_VIEWS, 5])
+    for i, (pos_i, h) in enumerate(zip(cur_pos, headings)):
+        x, y, z = pos_i
+        xyzhe[i, :, 0] = x
+        xyzhe[i, :, 1] = y
+        xyzhe[i, :, 2] = z
+        xyzhe[i, :, 3] = -np.arange(LIFT_VIEWS) * np.radians(30) + h
+        xyzhe[i, :, 4] = np.pi
+    return frames64(xyzhe.reshape(-1, 5)).astype(np.float32)
+
+
+def lift_intrinsics(projector):
+    """(fx, fy, cx, cy) of the trainer's PointCloud as its `forward` uses them: compute_intrinsic_matrix
+    (bev_utils.py:91-100) in float64, rounded to float32 by torch.Tensor.  Raises ValueError for a projector whose
+    `forward` bb_bev_lift_points does not reproduce: a feature map other than lift's 14 x 14, or a world_shift_origin
+    other than three float32 values."""
+    fmh, fmw, vfov = projector.fmh, projector.fmw, projector.vfov
+    if (fmh, fmw) != (LIFT_GRID, LIFT_GRID):
+        raise ValueError("lift reads 14 x 14 depth grids; the projector's feature map is %s x %s" % (fmh, fmw))
+    if not isinstance(vfov, (int, float)) or not 0.0 < vfov < math.pi:
+        raise ValueError("projector.vfov must be a field of view in (0, pi) radians, got %r" % (vfov,))
+    shift = projector.world_shift_origin
+    if not (torch.is_tensor(shift) and shift.dtype == torch.float32 and shift.numel() == 3 and shift.shape[-1] == 3):
+        raise ValueError("projector.world_shift_origin must be a float32 tensor of three values, got %r" % (shift,))
+    hfov = fmw / fmh * vfov
+    K = [fmw / (2.0 * math.tan(hfov / 2.0)), fmh / (2.0 * math.tan(vfov / 2.0)), fmw / 2.0, fmh / 2.0]
+    return tuple(torch.tensor(K, dtype=torch.float32).tolist())
+
+
+def ce_lift(trainer, cur_pos, cur_ori, rgb_grid, depth_grid):
+    """Drop-in for the VLN-CE trainer's `lift(cur_pos, cur_ori, rgb_grid, depth_grid)` (ss_trainer_BEV.py:386-410),
+    same (pc (B, 2352, 3), pc_mask (B, 2352), pc_feat (B, 2352, 768)).  The heading fan is `lift_frames` with the
+    trainer's own `heading_from_quaternion` (`_trainer_heading_fn`), uploaded in one copy; one `bb_bev_lift_points`
+    launch then does `PointCloud.forward` (bev_utils.py:349-378) on `depth_grid * 10` with the trainer's projector
+    (`lift_intrinsics`), the camera-to-world product in the kernel's fixed fp32 order where the reference calls bmm.
+    pc_feat is a view of rgb_grid, as in the reference.  depth_grid: contiguous float32 CUDA tensor of B * 12 * 196
+    values (the waypoint step's pano_depth_grid), read in place; rgb_grid on the same device.  Nothing in it
+    synchronises with the host.
+
+    Install on the trainer once it is built: graphs.install_ce_lift(trainer)."""
+    fx, fy, cx, cy = lift_intrinsics(trainer.projector)
+    B = len(cur_pos)
+    n = B * LIFT_VIEWS * LIFT_GRID * LIFT_GRID
+    if not (torch.is_tensor(depth_grid) and depth_grid.is_cuda and depth_grid.dtype == torch.float32
+            and depth_grid.is_contiguous() and depth_grid.numel() == n):
+        raise ValueError("depth_grid must be a contiguous float32 CUDA tensor of %d x 12 x 196 values, got %s"
+                         % (B, depth_grid.dtype if torch.is_tensor(depth_grid) else type(depth_grid)))
+    dev = depth_grid.device
+    if rgb_grid.device != dev or trainer.projector.world_shift_origin.device != dev:
+        raise ValueError("rgb_grid and projector.world_shift_origin must be on %s" % dev)
+    heading_from_quaternion = _trainer_heading_fn(trainer)
+    T = torch.from_numpy(lift_frames(cur_pos, [heading_from_quaternion(o) for o in cur_ori]))
+    T = T.pin_memory().to(dev, non_blocking=True)
+    shift = trainer.projector.world_shift_origin.reshape(3).contiguous()
+    pc, pc_mask = bev_nodes.bev_lift_points(depth_grid.view(-1, LIFT_GRID, LIFT_GRID), T, shift, 10.0, fx, fy, cx, cy)
+    pc_feat = rgb_grid.reshape(-1, LIFT_GRID, LIFT_GRID, LIFT_DIM).reshape(B, -1, LIFT_DIM)
+    return pc.view(B, -1, 3), pc_mask.view(B, -1), pc_feat
 
 
 def ce_nav_bev_variable(trainer, cur_vp, cur_pos, cur_ori):

@@ -1,7 +1,8 @@
-"""Tensor-level wrapper of `bb_bev_splat_nodes` (include/bevbert_b200.h): the agents' per-step BEV pooled straight from
-the navigation graph's node point clouds.  It lives beside `kernels.py` rather than in it because it keeps host state
-(the pinned launch tables); like every wrapper it only checks arguments, fills the table and launches, and raises
-without the CUDA library."""
+"""Tensor-level wrappers of the node point-cloud kernels (include/bevbert_b200.h): `bb_bev_splat_nodes`, the agents'
+per-step BEV pooled straight from the navigation graph's node clouds, and `bb_bev_lift_points`, which makes the VLN-CE
+trainer's node clouds.  The splat wrapper keeps host state (the pinned launch tables), which is why it lives beside
+`kernels.py` rather than in it; the lift wrapper sits with it because it produces the clouds the splat reads.  Every
+wrapper only checks arguments, fills a table where there is one and launches, and raises without the CUDA library."""
 import numpy as np
 import torch
 
@@ -101,3 +102,24 @@ def bev_splat_nodes(clouds, S_w2c, T_w2c, map_dim, map_res, y_clip=0.5, C=None):
     slot.mark_busy()
     _lib.check(rc, "bb_bev_splat_nodes")
     return bev, ob
+
+
+def bev_lift_points(depths, T_c2w, world_shift, depth_scale, fx, fy, cx, cy):
+    """World points of N depth views (bb_bev_lift_points): depths f32 (N, Hf, Wf) stored units, T_c2w f32 (N, 4, 4),
+    world_shift f32 (3,), all contiguous on one device -> (pts f32 (N, Hf*Wf, 3), no_depth bool (N, Hf*Wf))."""
+    for t, n in ((depths, "depths"), (T_c2w, "T_c2w"), (world_shift, "world_shift")):
+        _req(t, torch.float32, n)
+        if not t.is_contiguous():
+            raise ValueError("%s must be contiguous" % n)
+        if t.device != depths.device:
+            raise ValueError("%s must be on %s, got %s" % (n, depths.device, t.device))
+    if depths.dim() != 3 or T_c2w.shape != (depths.shape[0], 4, 4) or world_shift.shape != (3,):
+        raise ValueError("want depths (N, Hf, Wf), T_c2w (N, 4, 4) and world_shift (3,), got %s, %s and %s"
+                         % (tuple(depths.shape), tuple(T_c2w.shape), tuple(world_shift.shape)))
+    N, Hf, Wf = depths.shape
+    pts = torch.empty(N, Hf * Wf, 3, dtype=torch.float32, device=depths.device)
+    nod = torch.empty(N, Hf * Wf, dtype=torch.bool, device=depths.device)
+    _lib.check(_lib.load().bb_bev_lift_points(depths.data_ptr(), T_c2w.data_ptr(), N, Hf, Wf, depth_scale, fx, fy, cx,
+                                              cy, world_shift.data_ptr(), pts.data_ptr(), nod.data_ptr(), _stream()),
+               "bb_bev_lift_points")
+    return pts, nod

@@ -46,6 +46,27 @@ __device__ __forceinline__ int32_t bev_cell(float e0, float e1, float e2, bool n
   return bad ? -1 : (int32_t)(Df * gz + gx);
 }
 
+// depth pixel -> world point (bev_utils.py:130-131,167-172,198): z = d * depth_scale, x = z * ((col + 0.5 - cx) / fx),
+// y = z * ((row + 0.5 - cy) / fy), then each row of T (4x4 row major) dotted with (x, y, z, 1) left to right.
+// Returns the no-depth flag, z == 0 after the scale (bev_utils.py:371).
+__device__ __forceinline__ bool camera_to_world(float d, int row, int col, float depth_scale, float fx, float fy,
+                                                float cx, float cy, const float* T, float w[3]) {
+  const float z = __fmul_rn(d, depth_scale);  // depths * 10   (pretrain_cmt.py:125, ss_trainer_BEV.py:402)
+  const float xs = __fdiv_rn(__fsub_rn(__fadd_rn((float)col, 0.5f), cx), fx);  // bev_utils.py:130
+  const float ys = __fdiv_rn(__fsub_rn(__fadd_rn((float)row, 0.5f), cy), fy);  // bev_utils.py:131
+  const float x = __fmul_rn(z, xs);
+  const float y = __fmul_rn(z, ys);
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    float acc = __fmul_rn(T[j * 4 + 0], x);
+    acc = __fadd_rn(acc, __fmul_rn(T[j * 4 + 1], y));
+    acc = __fadd_rn(acc, __fmul_rn(T[j * 4 + 2], z));
+    acc = __fadd_rn(acc, T[j * 4 + 3]);
+    w[j] = acc;
+  }
+  return z == 0.0f;
+}
+
 // One thread per point.
 __global__ void lift_index_kernel(const float* __restrict__ depths, const float* __restrict__ T_c2w,
                                   const float* __restrict__ S_w2c, const float* __restrict__ T_w2c, int B, int V, int Hf,
@@ -62,23 +83,9 @@ __global__ void lift_index_kernel(const float* __restrict__ depths, const float*
   const int pix = pidx % (Hf * Wf);
   const int row = pix / Wf, col = pix % Wf;
 
-  const float z = __fmul_rn(depths[gid], depth_scale);  // depths * 10   (pretrain_cmt.py:125)
-  const bool no_depth = (z == 0.0f);                    // bev_utils.py:371
-  const float xs = __fdiv_rn(__fsub_rn(__fadd_rn((float)col, 0.5f), cx), fx);  // bev_utils.py:130
-  const float ys = __fdiv_rn(__fsub_rn(__fadd_rn((float)row, 0.5f), cy), fy);  // bev_utils.py:131
-  const float x = __fmul_rn(z, xs);
-  const float y = __fmul_rn(z, ys);
-  // camera -> world: T (4x4 row major) * (x, y, z, 1)   (bev_utils.py:198)
-  const float* T = T_c2w + ((long long)b * V + v) * 16;
   float w[3];
-#pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    float acc = __fmul_rn(T[j * 4 + 0], x);
-    acc = __fadd_rn(acc, __fmul_rn(T[j * 4 + 1], y));
-    acc = __fadd_rn(acc, __fmul_rn(T[j * 4 + 2], z));
-    acc = __fadd_rn(acc, T[j * 4 + 3]);
-    w[j] = acc;
-  }
+  const bool no_depth = camera_to_world(depths[gid], row, col, depth_scale, fx, fy, cx, cy,
+                                        T_c2w + ((long long)b * V + v) * 16, w);
   float e[3];
   ego_transform(w[0], w[1], w[2], S_w2c + (long long)b * 3, T_w2c + (long long)b * 16, e);
   if (pc_out) {
@@ -87,6 +94,38 @@ __global__ void lift_index_kernel(const float* __restrict__ depths, const float*
     pc_out[gid * 3 + 2] = e[2];
   }
   cell_idx[gid] = bev_cell(e[0], e[1], e[2], no_depth, D, res, half, y_clip);
+}
+
+// World points and no-depth mask of N depth views (PointCloud.forward, bev_utils.py:349-378, as the VLN-CE trainer's
+// `lift` calls it, ss_trainer_BEV.py:386-410): one thread per point, world point minus world_shift (3 floats).
+// The block's points are staged in shared memory so that the (n, 3) rows leave as consecutive floats.
+constexpr int LP_THREADS = 256;
+
+__global__ void __launch_bounds__(LP_THREADS)
+lift_points_kernel(const float* __restrict__ depths, const float* __restrict__ T_c2w, long long n, int HW, int Wf,
+                   float depth_scale, float fx, float fy, float cx, float cy, const float* __restrict__ world_shift,
+                   float* __restrict__ pts, uint8_t* __restrict__ no_depth) {
+  __shared__ float spts[LP_THREADS * 3];
+  bb::pdl_wait();
+  bb::pdl_trigger();
+  const long long base = (long long)blockIdx.x * LP_THREADS;
+  const long long gid = base + threadIdx.x;
+  if (gid < n) {
+    const long long view = gid / HW;
+    const int pix = (int)(gid - view * HW);
+    float w[3];
+    no_depth[gid] = camera_to_world(__ldg(depths + gid), pix / Wf, pix % Wf, depth_scale, fx, fy, cx, cy,
+                                    T_c2w + view * 16, w);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) spts[threadIdx.x * 3 + j] = __fsub_rn(w[j], __ldg(world_shift + j));  // :243
+  }
+  __syncthreads();
+  const long long nf = (n - base) * 3;  // floats this block owns
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int i = k * LP_THREADS + threadIdx.x;
+    if (i < nf) pts[base * 3 + i] = spts[i];
+  }
 }
 
 // Cell index of an ego-frame point cloud (PointCloud.project_bev called with a ready-made cloud: the agents gather
@@ -378,6 +417,25 @@ extern "C" int bb_bev_lift_index(const float* depths, const float* T_c2w, const 
       pc_out);
   count_launch();
   return check_launch("lift_index_kernel");
+}
+
+extern "C" int bb_bev_lift_points(const float* depths, const float* T_c2w, int N, int Hf, int Wf, float depth_scale,
+                                  float fx, float fy, float cx, float cy, const float* world_shift, float* pts,
+                                  uint8_t* no_depth, void* stream) {
+  using namespace bb;
+  if (!depths || !T_c2w || !world_shift || !pts || !no_depth) return set_error("bb_bev_lift_points: null argument");
+  if (((uintptr_t)depths | (uintptr_t)T_c2w | (uintptr_t)world_shift | (uintptr_t)pts) % 4 != 0)
+    return set_error("bb_bev_lift_points: float arguments must be 4-byte aligned");
+  if (N <= 0) return set_error("bb_bev_lift_points: N must be > 0");
+  if (Hf <= 0 || Wf <= 0 || (long long)Hf * Wf > INT32_MAX)
+    return set_error("bb_bev_lift_points: Hf * Wf must be positive and fit in 32 bits");
+  const long long n = (long long)N * Hf * Wf;
+  const long long blocks = (n + LP_THREADS - 1) / LP_THREADS;
+  if (blocks > INT32_MAX) return set_error("bb_bev_lift_points: too many points for one launch");
+  bb::launch_pdl(lift_points_kernel, (unsigned)blocks, LP_THREADS, 0, (cudaStream_t)stream, depths, T_c2w, n, Hf * Wf,
+                 Wf, depth_scale, fx, fy, cx, cy, world_shift, pts, no_depth);
+  count_launch();
+  return check_launch("lift_points_kernel");
 }
 
 extern "C" int bb_bev_cell_index(const float* pc, const uint8_t* no_depth, int64_t npoints, int map_dim, float map_res,

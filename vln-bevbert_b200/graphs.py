@@ -23,6 +23,7 @@ gradients); a step whose capture fails (a host synchronisation somewhere in forw
 `install_ce_replay` the VLN-CE policy's, `install_ce_rgb_encoder` the CE policy's CLIP RGB encoder,
 `install_ce_depth_encoder` its ResNet-50 depth encoder, and `install_ce_waypoint_predictor` the CE trainer's waypoint
 predictor.  `install_ce_gmap_features` builds the CE trainer's global-map image input on the kernels (no replay).
+`install_ce_lift` runs the CE trainer's `lift` (node point clouds) on the kernels (no replay).
 """
 import functools
 
@@ -572,6 +573,20 @@ def install_ce_gmap_features(trainer):
     net.forward = panorama_forward
     trainer._nav_gmap_variable = nav_gmap_variable
     return nav_gmap_variable
+
+
+def install_ce_lift(trainer):
+    """Replaces the CE trainer's `lift(cur_pos, cur_ori, rgb_grid, depth_grid)` with agent_bev.ce_lift: the heading fan
+    in one upload and PointCloud.forward in one bb_bev_lift_points launch, with no host synchronisation.  The projector
+    is checked here (ValueError if the kernel does not reproduce it) and again on every call.  update_node_pc,
+    gather_node_pc and _nav_bev_variable read the clouds as before.  -> the installed lift."""
+    from . import agent_bev
+    agent_bev.lift_intrinsics(trainer.projector)
+
+    def lift(cur_pos, cur_ori, rgb_grid, depth_grid):
+        return agent_bev.ce_lift(trainer, cur_pos, cur_ori, rgb_grid, depth_grid)
+    trainer.lift = lift
+    return lift
 
 
 class GraphedNavigation:
